@@ -101,6 +101,14 @@ template <typename T> B2_HD cx<T> ldg(const cx<T>* p) {
     return *p;
 #endif
 }
+// bring the line holding *p into L1 ahead of an ldg of it (no register is held while the line is in flight)
+template <typename T> B2_HD void prefetch_l1(const T* p) {
+#if defined(__CUDA_ARCH__)
+    asm volatile("prefetch.global.L1 [%0];" ::"l"(p));
+#else
+    (void)p;
+#endif
+}
 // large read-only tables that are streamed once per CTA (the N-entry inter-pass twiddle table): L2 only
 template <typename T> B2_HD cx<T> ldg_stream(const cx<T>* p) {
 #if defined(__CUDA_ARCH__)

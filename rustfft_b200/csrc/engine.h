@@ -78,17 +78,10 @@ struct Engine {
     using RL = typename G::RL;
     static constexpr int E = G::E;
 
-    // the table entries a stage loads per butterfly when the other factors are built as products (B2_TW_FEW): W^(k 2^i)
+    // warm L1 with the table entries stage S loads per butterfly when the other factors are built as products (B2_TW_FEW):
+    // W^(k 2^i) for thread (f, j) -- e.g. while the tile itself is still in flight
     template <int S>
-    struct TwRegs {
-        static constexpr int R = RL::get(S);
-        static constexpr int Q = E / R;
-        static constexpr int LG = ilog2_c(R);
-        cx<T> w[Q][LG > 0 ? LG : 1];
-    };
-    // prefetch them for thread (f, j) -- e.g. while the tile itself is still in flight
-    template <int S>
-    static B2_HD void load_tw(int j, const cx<T>* tw, TwRegs<S>& t) {
+    static B2_HD void prefetch_tw(int j, const cx<T>* tw) {
         constexpr int R = RL::get(S);
         constexpr int p = RL::product(S);
         constexpr int Q = E / R;
@@ -98,13 +91,13 @@ struct Engine {
             const int k = (p == 1) ? 0 : (i % p);
             const cx<T>* tp = tw + RL::tw_offset(S) + k;
             B2_UNROLL
-            for (int l = 0; l < TwRegs<S>::LG; ++l) t.w[u][l] = ldg(tp + ((1 << l) - 1) * p);
+            for (int r = 1; r < R; r <<= 1) prefetch_l1(tp + (r - 1) * p);
         }
     }
 
     // one stage: consumes v (slot q <-> element j + TP*q), produces either smem (not last) or v
     template <int S>
-    static B2_HD void stage(int f, int j, cx<T> (&v)[E], cx<T>* smem, const cx<T>* tw, const TwRegs<S>* pre = nullptr) {
+    static B2_HD void stage(int f, int j, cx<T> (&v)[E], cx<T>* smem, const cx<T>* tw) {
         constexpr int R = RL::get(S);
         constexpr int p = RL::product(S);
         constexpr int Q = E / R;
@@ -126,7 +119,7 @@ struct Engine {
                     // log2 R correctly rounded table entries): log2 R loads instead of R - 1 through the LSU
                     cx<T> w[R];
                     B2_UNROLL
-                    for (int r = 1, l = 0; r < R; r <<= 1, ++l) w[r] = pre ? pre->w[u][l] : ldg(t + (r - 1) * p);
+                    for (int r = 1; r < R; r <<= 1) w[r] = ldg(t + (r - 1) * p);
                     B2_UNROLL
                     for (int r = 3; r < R; ++r)
                         if (r & (r - 1)) {
@@ -204,12 +197,6 @@ struct Engine {
         } else {
             stage<P / 2>(f, j, v, smem, tw);
         }
-    }
-    // the last phase with its twiddles already in registers (load_tw<NS-1>)
-    static B2_HD void last_phase_pre(int tid, cx<T> (&v)[E], cx<T>* smem, const cx<T>* tw, const TwRegs<G::NS - 1>& pre) {
-        int f, j;
-        owner<NPHASE - 1>(tid, f, j);
-        stage<G::NS - 1>(f, j, v, smem, tw, &pre);
     }
 };
 

@@ -12,6 +12,8 @@
 //                         dense tile in the same buffer;
 //     1 storer thread     TMA-stores finished tiles, frees the stage once the store has read it, publishes the
 //                         "pass-A tile landed" counters;
+// the scheduler, producer and storer warps (plus one idle warp) form one warpgroup that gives up registers with
+// setmaxnreg, so that the consumer warpgroups can hold a tile's 32 values per thread without spilling;
 // so the load of tile i+2, the butterflies of tiles i and i+1 and the store of tile i-1 overlap inside one SM, there
 // are no launches between tiles, and the device mixes HBM reads (pass-A tiles) with HBM writes (pass-B tiles) at tile
 // granularity.  Ticket order = FlowSched (kernels.h): round r holds the pass-A tiles of transform r interleaved with
@@ -36,7 +38,19 @@ struct FusedKernel {
     static_assert(KA::NT == KB::NT, "both passes use the same consumer-group size");
     static_assert(KA::TILE_BYTES == KB::TILE_BYTES, "both passes move tiles of the same size");
     static_assert(NTG % 32 == 0 && NSTAGE <= 8 && NG <= 8, "geometry");
-    static constexpr int NT = NG * NTG + 96;  // + producer warp + storer warp + scheduler warp
+    // consumer groups first, then ONE service warpgroup (producer, storer, scheduler, spare warp): setmaxnreg acts on whole
+    // warpgroups, so the service roles can hand their registers to the consumers only if no consumer warp shares their group
+    static_assert(NG * NTG % 128 == 0, "consumer groups fill whole warpgroups");
+    static constexpr int NT = NG * NTG + 128;
+    static constexpr int SVC_WARP = NG * NTG / 32;  // first warp of the service warpgroup
+    // register budgets: the launch grants every thread LAUNCH_REGS (__launch_bounds__(NT, 1) over the 64 K register file,
+    // rounded down to the allocation granule of 8); the service warpgroup shrinks to SVC_REGS and the consumers grow to
+    // CONS_REGS, claiming no more than the service warpgroup released
+    static constexpr int LAUNCH_REGS = 65536 / NT / 8 * 8;
+    static constexpr int SVC_REGS = 32;  // 24 spills in the scheduler and producer loops
+    static constexpr int CONS_REGS = (LAUNCH_REGS * NT - SVC_REGS * 128) / (NG * NTG) / 8 * 8;
+    static_assert(CONS_REGS * NG * NTG + SVC_REGS * 128 <= LAUNCH_REGS * NT && CONS_REGS >= LAUNCH_REGS && CONS_REGS <= 256,
+                  "setmaxnreg budgets must not overcommit the registers the launch granted");
     static constexpr int NQ = 2;              // tiles the scheduler may run ahead of the producer
     static constexpr size_t STAGE_BYTES = ((KA::SMEM_BYTES > KB::SMEM_BYTES ? KA::SMEM_BYTES : KB::SMEM_BYTES) + 127) / 128 * 128;
     static constexpr size_t CTRL_BYTES = 512;  // 4 * NSTAGE + 2 * NQ mbarriers, (NSTAGE + NQ) x {kind, tile, slot, -}
@@ -156,157 +170,162 @@ run_fused(const __grid_constant__ typename FusedKernel<KA, KB, NG, NS>::Params p
     // tiles the scheduler may run ahead of the producer: 1 (measured best: a ticket claimed early is a tile others may wait for)
     const uint32_t nq = (p.flags & 64u) ? (uint32_t)FK::NQ : 1u;
 
-    if (warp == NG * NTG / 32 + 2) {
-        // ---------------- scheduler ----------------
-        // Draws tickets, resolves their dependencies and hands ready-to-load tiles to the producer through a small queue.
-        // Everything with a round trip to L2 in it (ticket counter, dependency counters) lives in THIS thread: measured with
-        // the pipeline trace (tools/fused_trace.py), the same work inside the producer thread kept a freed stage empty for 1.4 us.
-        if (lane == 0) {
-            uint32_t k = 0;
-            uint32_t ticket = atomicAdd(p.ctl, 1u);
-            while (ticket < sc.total) {
-                int kind;
-                uint32_t t, tile;
-                bool valid;
-                sc.decode(ticket, kind, t, tile, valid);
-                const uint32_t next = atomicAdd(p.ctl, 1u);  // in flight while this ticket's dependency is resolved
-                if (valid) {
-                    const FlowDep d = flow_dep(sc, p.ctl, ticket);
-                    if (d.ptr != nullptr && ld_acquire_u32(d.ptr) < d.target) fused_spin(p.ctl, d.ptr, d.target);
-                    // the acquire above (generic proxy) -> the TMA accesses of the slot (async proxy), issued by the producer and the
-                    // storer after they have synchronised with this thread through the queue.  The fence sits HERE because in the
-                    // producer it also waited for that thread's outstanding tile loads (measured: +0.7..1.1 us per tile).
-                    if (d.ptr != nullptr) tma::fence_proxy_async_all();
-                    const uint32_t q = k % nq, qph = (k / nq) & 1u;
-                    tma::mbar_wait(&q_empty[q], qph ^ 1u);
-                    qent[4 * q + 0] = (uint32_t)kind;
-                    qent[4 * q + 1] = kind == 0 ? t * sc.TA + tile : t * sc.TB + tile;
-                    qent[4 * q + 2] = t % sc.ring_w;
-                    tma::mbar_arrive(&q_full[q]);
-                    ++k;
+    if (warp >= FK::SVC_WARP) {
+        // each budget change sits inside its branch, so that ptxas allocates every role's code under that role's budget
+        tma::setmaxnreg_dec<FK::SVC_REGS>();
+        if (warp == FK::SVC_WARP + 2) {
+            // ---------------- scheduler ----------------
+            // Draws tickets, resolves their dependencies and hands ready-to-load tiles to the producer through a small queue.
+            // Everything with a round trip to L2 in it (ticket counter, dependency counters) lives in THIS thread: measured with
+            // the pipeline trace (tools/fused_trace.py), the same work inside the producer thread kept a freed stage empty for 1.4 us.
+            if (lane == 0) {
+                uint32_t k = 0;
+                uint32_t ticket = atomicAdd(p.ctl, 1u);
+                while (ticket < sc.total) {
+                    int kind;
+                    uint32_t t, tile;
+                    bool valid;
+                    sc.decode(ticket, kind, t, tile, valid);
+                    const uint32_t next = atomicAdd(p.ctl, 1u);  // in flight while this ticket's dependency is resolved
+                    if (valid) {
+                        const FlowDep d = flow_dep(sc, p.ctl, ticket);
+                        if (d.ptr != nullptr && ld_acquire_u32(d.ptr) < d.target) fused_spin(p.ctl, d.ptr, d.target);
+                        // the acquire above (generic proxy) -> the TMA accesses of the slot (async proxy), issued by the producer and the
+                        // storer after they have synchronised with this thread through the queue.  The fence sits HERE because in the
+                        // producer it also waited for that thread's outstanding tile loads (measured: +0.7..1.1 us per tile).
+                        if (d.ptr != nullptr) tma::fence_proxy_async_all();
+                        const uint32_t q = k % nq, qph = (k / nq) & 1u;
+                        tma::mbar_wait(&q_empty[q], qph ^ 1u);
+                        qent[4 * q + 0] = (uint32_t)kind;
+                        qent[4 * q + 1] = kind == 0 ? t * sc.TA + tile : t * sc.TB + tile;
+                        qent[4 * q + 2] = t % sc.ring_w;
+                        tma::mbar_arrive(&q_full[q]);
+                        ++k;
+                    }
+                    ticket = next;
                 }
-                ticket = next;
-            }
-            const uint32_t q = k % nq, qph = (k / nq) & 1u;
-            tma::mbar_wait(&q_empty[q], qph ^ 1u);
-            qent[4 * q + 0] = 2u;  // end of work
-            tma::mbar_arrive(&q_full[q]);
-        }
-    } else if (warp == NG * NTG / 32) {
-        // ---------------- producer ----------------
-        if (lane == 0) {
-            uint32_t i = 0;
-            FusedTrace tr;
-            tr.init(p.trace, 0);
-            const unsigned long long pol_a = (p.flags & 2u) ? l2_evict_first() : 0ull, pol_b = (p.flags & 4u) ? l2_evict_first() : 0ull;
-            for (uint32_t k = 0;; ++k) {
                 const uint32_t q = k % nq, qph = (k / nq) & 1u;
-                tma::mbar_wait(&q_full[q], qph);
-                const uint32_t kind = qent[4 * q + 0], bid = qent[4 * q + 1], slot = qent[4 * q + 2];
-                tma::mbar_arrive(&q_empty[q]);
-                if (kind == 2u) break;
-                const uint32_t s = i % NS, ph = (i / NS) & 1u;
-                tr.stamp(0x10u | kind);              // a resolved ticket in hand
-                tma::mbar_wait(&empty[s], ph ^ 1u);  // (passes at once for the first NS tiles)
-                tr.stamp(0x20u | s);                 // stage free
-                info[4 * s + 0] = kind;
-                info[4 * s + 1] = bid;
-                info[4 * s + 2] = slot;
-                tma::mbar_arrive(&meta[s]);
-                if (kind == 0u)
-                    KA::issue_load(p.a, bid, stage_buf(s), &full[s], pol_a);
-                else
-                    KB::issue_load(p.b, bid, stage_buf(s), &full[s], pol_b);
-                tr.stamp(0x30u | s);  // load queued
-                ++i;
+                tma::mbar_wait(&q_empty[q], qph ^ 1u);
+                qent[4 * q + 0] = 2u;  // end of work
+                tma::mbar_arrive(&q_full[q]);
             }
-            for (int g = 0; g < NG; ++g, ++i) {  // one end marker per consumer group
-                const uint32_t s = i % NS, ph = (i / NS) & 1u;
-                tma::mbar_wait(&empty[s], ph ^ 1u);
-                info[4 * s + 0] = 2u;
-                tma::mbar_arrive(&meta[s]);
-            }
-            tr.finish();
-        }
-    } else if (warp == NG * NTG / 32 + 1) {
-        // ---------------- storer ----------------
-        // Finished tiles that leave through shared memory (all pass-B tiles; pass-A tiles too when the ring is not tile-major)
-        // complete their stage's `outf` barrier in no particular order: poll the stages.
-        if (lane == 0) {
-            uint32_t* pending = nullptr;  // ready counter of the last pass-A tile stored, not yet published
-            const unsigned long long pol_a = (p.flags & 8u) ? l2_evict_last() : 0ull, pol_b = (p.flags & 16u) ? l2_evict_first() : 0ull;
-            FusedTrace tr;
-            tr.init(p.trace, 1);
-            uint32_t sph = 0;  // bit s: parity of the next completion of outf[s]
-            uint32_t held = 0xffffffffu;  // stage whose store is queued but not yet known to have been read (two-in-flight mode)
-            int ends = 0;
-            uint32_t idle = 0;
-            while (ends < NG) {
-                bool any = false;
-                for (uint32_t s = 0; s < (uint32_t)NS; ++s) {
-                    if (!tma::mbar_test(&outf[s], (sph >> s) & 1u)) continue;
-                    sph ^= 1u << s;
-                    any = true;
-                    const uint32_t kind = info[4 * s + 0], bid = info[4 * s + 1], slot = info[4 * s + 2];
-                    if (kind == 2u) {
-                        ++ends;
-                        continue;
-                    }
-                    tr.stamp(0x40u | s);  // finished tile seen
+        } else if (warp == FK::SVC_WARP) {
+            // ---------------- producer ----------------
+            if (lane == 0) {
+                uint32_t i = 0;
+                FusedTrace tr;
+                tr.init(p.trace, 0);
+                const unsigned long long pol_a = (p.flags & 2u) ? l2_evict_first() : 0ull, pol_b = (p.flags & 4u) ? l2_evict_first() : 0ull;
+                for (uint32_t k = 0;; ++k) {
+                    const uint32_t q = k % nq, qph = (k / nq) & 1u;
+                    tma::mbar_wait(&q_full[q], qph);
+                    const uint32_t kind = qent[4 * q + 0], bid = qent[4 * q + 1], slot = qent[4 * q + 2];
+                    tma::mbar_arrive(&q_empty[q]);
+                    if (kind == 2u) break;
+                    const uint32_t s = i % NS, ph = (i / NS) & 1u;
+                    tr.stamp(0x10u | kind);              // a resolved ticket in hand
+                    tma::mbar_wait(&empty[s], ph ^ 1u);  // (passes at once for the first NS tiles)
+                    tr.stamp(0x20u | s);                 // stage free
+                    info[4 * s + 0] = kind;
+                    info[4 * s + 1] = bid;
+                    info[4 * s + 2] = slot;
+                    tma::mbar_arrive(&meta[s]);
                     if (kind == 0u)
-                        KA::issue_store(p.a, bid, stage_buf(s), pol_a);
+                        KA::issue_load(p.a, bid, stage_buf(s), &full[s], pol_a);
                     else
-                        KB::issue_store(p.b, bid, stage_buf(s), pol_b);
-                    tma::bulk_commit();
-                    if (pending != nullptr) {  // every group but the one just committed has completed
-                        tma::bulk_wait<1>();
-                        tma::fence_proxy_async_all();
-                        red_release_add1(pending);
-                        pending = nullptr;
+                        KB::issue_load(p.b, bid, stage_buf(s), &full[s], pol_b);
+                    tr.stamp(0x30u | s);  // load queued
+                    ++i;
+                }
+                for (int g = 0; g < NG; ++g, ++i) {  // one end marker per consumer group
+                    const uint32_t s = i % NS, ph = (i / NS) & 1u;
+                    tma::mbar_wait(&empty[s], ph ^ 1u);
+                    info[4 * s + 0] = 2u;
+                    tma::mbar_arrive(&meta[s]);
+                }
+                tr.finish();
+            }
+        } else if (warp == FK::SVC_WARP + 1) {
+            // ---------------- storer ----------------
+            // Finished tiles that leave through shared memory (all pass-B tiles; pass-A tiles too when the ring is not tile-major)
+            // complete their stage's `outf` barrier in no particular order: poll the stages.
+            if (lane == 0) {
+                uint32_t* pending = nullptr;  // ready counter of the last pass-A tile stored, not yet published
+                const unsigned long long pol_a = (p.flags & 8u) ? l2_evict_last() : 0ull, pol_b = (p.flags & 16u) ? l2_evict_first() : 0ull;
+                FusedTrace tr;
+                tr.init(p.trace, 1);
+                uint32_t sph = 0;  // bit s: parity of the next completion of outf[s]
+                uint32_t held = 0xffffffffu;  // stage whose store is queued but not yet known to have been read (two-in-flight mode)
+                int ends = 0;
+                uint32_t idle = 0;
+                while (ends < NG) {
+                    bool any = false;
+                    for (uint32_t s = 0; s < (uint32_t)NS; ++s) {
+                        if (!tma::mbar_test(&outf[s], (sph >> s) & 1u)) continue;
+                        sph ^= 1u << s;
+                        any = true;
+                        const uint32_t kind = info[4 * s + 0], bid = info[4 * s + 1], slot = info[4 * s + 2];
+                        if (kind == 2u) {
+                            ++ends;
+                            continue;
+                        }
+                        tr.stamp(0x40u | s);  // finished tile seen
+                        if (kind == 0u)
+                            KA::issue_store(p.a, bid, stage_buf(s), pol_a);
+                        else
+                            KB::issue_store(p.b, bid, stage_buf(s), pol_b);
+                        tma::bulk_commit();
+                        if (pending != nullptr) {  // every group but the one just committed has completed
+                            tma::bulk_wait<1>();
+                            tma::fence_proxy_async_all();
+                            red_release_add1(pending);
+                            pending = nullptr;
+                        }
+                        tr.stamp(0x50u | s);       // store queued (+ previous pass-A tile published)
+                        if (p.flags & 128u) {
+                            // keep the store engine fed: the previous store's stage is released once this one is queued behind it
+                            if (held != 0xffffffffu) {
+                                tma::bulk_wait_read<1>();
+                                tma::mbar_arrive(&empty[held]);
+                                tr.stamp(0x60u | held);
+                            }
+                            held = s;
+                        } else {
+                            tma::bulk_wait_read<0>();  // the buffer may be refilled
+                            tma::mbar_arrive(&empty[s]);
+                            tr.stamp(0x60u | s);  // stage released
+                        }
+                        if (kind == 0u) pending = ready + slot;
                     }
-                    tr.stamp(0x50u | s);       // store queued (+ previous pass-A tile published)
-                    if (p.flags & 128u) {
-                        // keep the store engine fed: the previous store's stage is released once this one is queued behind it
+                    if (!any) {
                         if (held != 0xffffffffu) {
-                            tma::bulk_wait_read<1>();
+                            tma::bulk_wait_read<0>();
                             tma::mbar_arrive(&empty[held]);
                             tr.stamp(0x60u | held);
+                            held = 0xffffffffu;
                         }
-                        held = s;
+                        if (pending != nullptr) {  // idle: other CTAs (or this CTA's own scheduler) may be waiting for that tile
+                            tma::bulk_wait<0>();
+                            tma::fence_proxy_async_all();
+                            red_release_add1(pending);
+                            pending = nullptr;
+                        }
+                        __nanosleep(idle < 8 ? 32 : 128);
+                        ++idle;
                     } else {
-                        tma::bulk_wait_read<0>();  // the buffer may be refilled
-                        tma::mbar_arrive(&empty[s]);
-                        tr.stamp(0x60u | s);  // stage released
+                        idle = 0;
                     }
-                    if (kind == 0u) pending = ready + slot;
                 }
-                if (!any) {
-                    if (held != 0xffffffffu) {
-                        tma::bulk_wait_read<0>();
-                        tma::mbar_arrive(&empty[held]);
-                        tr.stamp(0x60u | held);
-                        held = 0xffffffffu;
-                    }
-                    if (pending != nullptr) {  // idle: other CTAs (or this CTA's own scheduler) may be waiting for that tile
-                        tma::bulk_wait<0>();
-                        tma::fence_proxy_async_all();
-                        red_release_add1(pending);
-                        pending = nullptr;
-                    }
-                    __nanosleep(idle < 8 ? 32 : 128);
-                    ++idle;
-                } else {
-                    idle = 0;
+                tma::bulk_wait<0>();
+                if (pending != nullptr) {
+                    tma::fence_proxy_async_all();
+                    red_release_add1(pending);
                 }
+                tr.finish();
             }
-            tma::bulk_wait<0>();
-            if (pending != nullptr) {
-                tma::fence_proxy_async_all();
-                red_release_add1(pending);
-            }
-            tr.finish();
-        }
+        }  // warp SVC_WARP + 3 only completes the warpgroup
     } else {
+        tma::setmaxnreg_inc<FK::CONS_REGS>();
         // ---------------- consumers ----------------
         const int g = warp / (NTG / 32);
         const int ltid = tid - g * NTG;

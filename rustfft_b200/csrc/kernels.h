@@ -1264,14 +1264,14 @@ struct TmaTileKernel {
     // slab (transform slot) a tile is read from / written to
     static B2_HD uint32_t zin(const Params& p, uint32_t b) { return (ROLE == 1 && p.ring_w) ? (p.z_in + b) % p.ring_w : p.z_in + b; }
     static B2_HD uint32_t zout(const Params& p, uint32_t b) { return (ROLE == 0 && p.ring_w) ? (p.z_out + b) % p.ring_w : p.z_out + b; }
-    // tables fetched while the tile is in flight (f32, two-stage tiles): the last stage's twiddles and, for pass B,
-    // the row's inter-pass twiddles -- the round-1 capture of these kernels had long_scoreboard (table loads issued
-    // right before their use) as the top stall
+    // tables fetched while the tile is in flight (f32, two-stage tiles): the last stage's twiddles (into L1 only: held in
+    // registers through phases 0 and 1 they made the fused kernel's consumers spill) and, for pass B, the row's
+    // inter-pass twiddles -- the round-1 capture of these kernels had long_scoreboard (table loads issued right before
+    // their use) as the top stall
     static constexpr bool PRE = (G::NS == 2) && sizeof(T) == 4 && ((RL_last_pow2<G>::value));
     static constexpr int LGE = ilog2_c(G::E);
     struct Regs {
         cx<T> v[G::E];
-        typename Eng::template TwRegs<G::NS - 1> twl;
         cx<T> rw[LGE + 1];  // ROLE 1: W^(k1 j), W^(k1 TP 2^i)
     };
     struct Where { uint32_t b, c0; };  // transform of the launch, first column (ROLE 0) / first row (ROLE 1) of the tile
@@ -1279,7 +1279,7 @@ struct TmaTileKernel {
         if constexpr (PRE) {
             int f, j;
             Eng::out_owner(tid, f, j);
-            Eng::template load_tw<G::NS - 1>(j, p.tw, r.twl);
+            Eng::template prefetch_tw<G::NS - 1>(j, p.tw);
             if (ROLE == 1) {
                 const Where w = where(p, bid);
                 Eng::template owner<0>(tid, f, j);
@@ -1392,12 +1392,13 @@ struct TmaTileKernel {
                     const cx<T> a = PRE ? r.rw[0] : ldg_stream(t);
                     B2_UNROLL
                     for (int q = 1, l = 1; q < G::E; q <<= 1, ++l) wq[q] = PRE ? r.rw[l] : ldg_stream(t - j + G::TP * q);
-                    B2_UNROLL
-                    for (int q = 3; q < G::E; ++q)
-                        if (q & (q - 1)) wq[q] = cmul(wq[hibit(q)], wq[q - hibit(q)]);
                     r.v[0] = cmul(at(0), a);
+                    // each product twiddle next to its first use: the upper half (q >= E/2) is never a factor, so it dies at once
                     B2_UNROLL
-                    for (int q = 1; q < G::E; ++q) r.v[q] = cmul(at(q), cmul(a, wq[q]));
+                    for (int q = 1; q < G::E; ++q) {
+                        if (q & (q - 1)) wq[q] = cmul(wq[hibit(q)], wq[q - hibit(q)]);
+                        r.v[q] = cmul(at(q), cmul(a, wq[q]));
+                    }
                 } else
 #endif
                 {
@@ -1424,10 +1425,7 @@ struct TmaTileKernel {
                     }
                 }
             }
-            if constexpr (P == NPHASE - 2 && PRE)
-                Eng::last_phase_pre(tid, r.v, buf, p.tw, r.twl);
-            else
-                Eng::template phase<P - 1>(tid, r.v, buf, p.tw);
+            Eng::template phase<P - 1>(tid, r.v, buf, p.tw);
             if constexpr (P == NPHASE - 2) {
                 int f, j;
                 Eng::out_owner(tid, f, j);

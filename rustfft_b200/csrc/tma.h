@@ -126,6 +126,10 @@ template <int N> B2_D void bulk_wait_read() { asm volatile("cp.async.bulk.wait_g
 B2_D void named_bar_sync(int id, int count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }
 B2_D void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 B2_D void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+// per-thread register budget of the calling warpgroup (every thread of all four warps executes the same one); REGS a
+// multiple of 8 in [24, 256].  `dec` returns registers to the CTA's pool, `inc` blocks until the pool can supply them.
+template <int REGS> B2_D void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(REGS)); }
+template <int REGS> B2_D void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(REGS)); }
 
 }  // namespace tma
 }  // namespace b2
