@@ -162,6 +162,33 @@ int b200fft_plan2d_destroy(b200fft_plan2d* plan);
 int b200fft_exec2d_device(const b200fft_plan2d* plan, const void* d_in, void* d_out, uint64_t batch, void* cuda_stream);
 int b200fft_exec2d_host(const b200fft_plan2d* plan, const void* in, void* out, uint64_t batch);
 
+/* Batched FFT convolution (SURVEY 8(f).4; what scipy.signal.fftconvolve / oaconvolve do): every row of a batch of rows of
+ * signal_len samples, contiguous, is convolved with ONE filter of filter_len taps fixed at plan time.  Plain sums, no scaling;
+ * the result equals scipy.signal.fftconvolve(row, filter, mode):
+ *   FULL   signal_len + filter_len - 1 outputs, output t = full-convolution index t
+ *   SAME   signal_len outputs starting at full index (filter_len - 1) / 2 (scipy's centring)
+ *   VALID  signal_len - filter_len + 1 outputs starting at full index filter_len - 1; needs signal_len >= filter_len
+ * Domains: COMPLEX rows and filter of float2 / double2; REAL rows and filter of float / double, real output (two rows share one
+ * complex transform).  Cross-correlation of x with h is the convolution of x with conj(h[::-1]) (the reversed, conjugated filter).
+ * filter: host memory, filter_len elements, 1 <= filter_len <= 2048 (B200FFT_ERR_UNSUPPORTED otherwise).  One launch and one pass
+ * over device memory per call, any signal length (overlap-save: blocks of M = 256..4096 points, M - filter_len + 1 outputs each,
+ * FFT -> * FFT(filter) -> inverse FFT inside one CTA).  No workspace.  Out of place only: overlapping input and output ranges are
+ * B200FFT_ERR_INVALID_ARG.  signal_len == 0 or batch == 0 is a silent no-op.  Plans are immutable and thread safe. */
+typedef struct b200fft_conv_plan b200fft_conv_plan;
+enum { B200FFT_CONV_FULL = 0, B200FFT_CONV_SAME = 1, B200FFT_CONV_VALID = 2 };
+enum { B200FFT_CONV_COMPLEX = 0, B200FFT_CONV_REAL = 1 };
+int b200fft_conv_plan_create(b200fft_conv_plan** out, uint64_t signal_len, const void* filter, uint64_t filter_len, int mode,
+                             int domain, int precision, int device);
+int b200fft_conv_plan_destroy(b200fft_conv_plan* plan);
+/* Samples per output row (0 for a NULL plan). */
+uint64_t b200fft_conv_output_len(const b200fft_conv_plan* plan);
+/* e.g. "OverlapSave{n=100000,m=255,M=2048,L=1794,full,real}".  Returns length or <0. */
+int b200fft_conv_describe(const b200fft_conv_plan* plan, char* buf, uint64_t cap);
+/* d_in: batch * signal_len samples, d_out: batch * output_len samples on the plan's device; asynchronous on `cuda_stream`. */
+int b200fft_conv_device(const b200fft_conv_plan* plan, const void* d_in, void* d_out, uint64_t batch, void* cuda_stream);
+/* Same on host memory, synchronous (plain copies in and out, not pipelined). */
+int b200fft_conv_host(const b200fft_conv_plan* plan, const void* in, void* out, uint64_t batch);
+
 /* Message of the last failing call on this thread ("" if none). */
 const char* b200fft_last_error(void);
 /* Library build string: "b200fft <version> sm_90a" */

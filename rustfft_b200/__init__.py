@@ -26,7 +26,8 @@ from typing import Dict, Optional, Tuple
 
 import numpy as np
 
-__all__ = ["FftDirection", "FftPlanner", "Fft", "Library", "FftError", "Recipe", "RealFftPlanner", "RealFft", "Fft2d", "default_library", "shard_range"]
+__all__ = ["FftDirection", "FftPlanner", "Fft", "Library", "FftError", "Recipe", "RealFftPlanner", "RealFft", "Fft2d", "FftConvolution", "default_library",
+           "shard_range"]
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 # B200FFT_LIB: load another build of the same C ABI (A/B measurements of kernel variants; tools/ab_two_pass.py)
@@ -127,6 +128,8 @@ class Library:
         "b200fft_real_plan_create", "b200fft_real_plan_destroy", "b200fft_real_workspace_bytes", "b200fft_real_forward_device",
         "b200fft_real_inverse_device", "b200fft_real_forward_host", "b200fft_real_inverse_host",
         "b200fft_plan2d_create", "b200fft_plan2d_destroy", "b200fft_exec2d_device", "b200fft_exec2d_host",
+        "b200fft_conv_plan_create", "b200fft_conv_plan_destroy", "b200fft_conv_output_len", "b200fft_conv_describe",
+        "b200fft_conv_device", "b200fft_conv_host",
     ]
 
     def __init__(self, path: str = DEFAULT_LIB_PATH):
@@ -170,6 +173,13 @@ class Library:
         c.b200fft_plan2d_destroy.argtypes = [vp]
         c.b200fft_exec2d_device.argtypes = [vp, vp, vp, u64, vp]
         c.b200fft_exec2d_host.argtypes = [vp, vp, vp, u64]
+        c.b200fft_conv_plan_create.argtypes = [ctypes.POINTER(vp), u64, vp, u64, i32, i32, i32, i32]
+        c.b200fft_conv_plan_destroy.argtypes = [vp]
+        c.b200fft_conv_output_len.argtypes = [vp]
+        c.b200fft_conv_output_len.restype = u64
+        c.b200fft_conv_describe.argtypes = [vp, ctypes.c_char_p, u64]
+        c.b200fft_conv_device.argtypes = [vp, vp, vp, u64, vp]
+        c.b200fft_conv_host.argtypes = [vp, vp, vp, u64]
 
     def device_count(self) -> int:
         n = ctypes.c_int(0)
@@ -397,6 +407,11 @@ class FftPlanner:
         """2-D transform of [height][width] images: the width-point plan over the rows, one strided pass down the columns."""
         return Fft2d(self._lib, height, width, direction, self._precision, self.device)
 
+    def plan_convolution(self, filter, signal_len: int, mode: str = "full") -> "FftConvolution":
+        """Convolution of complex rows of signal_len samples with `filter` (1-D, 1..2048 taps); see FftConvolution (not cached:
+        the filter is data)."""
+        return FftConvolution(self._lib, filter, signal_len, mode, False, self._precision, self.device)
+
     def plan_fft_forward(self, len: int) -> Fft:
         return self.plan_fft(len, FftDirection.Forward)
 
@@ -532,6 +547,99 @@ class RealFftPlanner:
             if f is None:
                 f = self._cache[int(len)] = RealFft(self._lib, int(len), self._precision, self.device)
             return f
+
+    def plan_convolution(self, filter, signal_len: int, mode: str = "full") -> FftConvolution:
+        """Convolution of real rows of signal_len samples with the real `filter` (1-D, 1..2048 taps); see FftConvolution (not
+        cached: the filter is data)."""
+        return FftConvolution(self._lib, filter, signal_len, mode, True, self._precision, self.device)
+
+
+class FftConvolution:
+    """Batched FFT convolution with one filter fixed at plan time: every contiguous row of signal_len samples becomes
+    scipy.signal.fftconvolve(row, filter, mode) -- plain sums, no scaling.  mode "full" (signal_len + m - 1 outputs), "same"
+    (signal_len, scipy's centring) or "valid" (signal_len - m + 1, needs signal_len >= m).  Complex rows and filter from
+    FftPlanner.plan_convolution, real ones from RealFftPlanner.plan_convolution.  Cross-correlation with h is the convolution
+    with np.conj(h[::-1]).
+
+    One launch and one pass over device memory (overlap-save inside one CTA per block), out of place only.  numpy arrays go
+    through the synchronous host entry point, torch CUDA tensors through the device one (asynchronous on torch's current
+    stream).  Immutable and safe to call from many threads."""
+
+    MODES = {"full": 0, "same": 1, "valid": 2}
+
+    def __init__(self, lib: Library, filter, signal_len: int, mode: str, real: bool, precision: int, device: int):
+        if mode not in self.MODES:
+            raise FftError(-1, f"unknown convolution mode {mode!r}: expected one of {sorted(self.MODES)}")
+        self._lib, self._real, self._precision, self.device, self.mode = lib, bool(real), precision, device, mode
+        self._signal_len = int(signal_len)
+        if real and np.iscomplexobj(filter):
+            raise TypeError("a real convolution plan needs a real filter")
+        h = np.ascontiguousarray(np.asarray(filter), dtype=self.dtype)
+        if h.ndim != 1:
+            raise TypeError("the filter must be 1-D")
+        self._h = ctypes.c_void_p()
+        lib.check(lib.c.b200fft_conv_plan_create(ctypes.byref(self._h), self._signal_len, h.ctypes.data, h.size, self.MODES[mode],
+                                                 1 if real else 0, precision, device))
+        self._out_len = int(lib.c.b200fft_conv_output_len(self._h))
+
+    def __del__(self):
+        h, self._h = getattr(self, "_h", None), None
+        if h:
+            try:
+                self._lib.c.b200fft_conv_plan_destroy(h)
+            except Exception:
+                pass
+
+    @property
+    def dtype(self):
+        if self._real:
+            return np.float32 if self._precision == F32 else np.float64
+        return np.complex64 if self._precision == F32 else np.complex128
+
+    def signal_len(self) -> int:
+        return self._signal_len
+
+    def output_len(self) -> int:
+        return self._out_len
+
+    def describe(self) -> str:
+        buf = ctypes.create_string_buffer(256)
+        rc = self._lib.c.b200fft_conv_describe(self._h, buf, len(buf))
+        if rc < 0:
+            self._lib.check(rc)
+        return buf.value.decode()
+
+    def _batch(self, n_in: int, n_out: int) -> int:
+        n, o = self._signal_len, self._out_len
+        if n == 0:
+            return 0
+        if n_in % n or n_out != n_in // n * o:
+            raise FftError(-6, f"FftConvolution: input holds {n_in} samples, output {n_out}: expected batch * {n} and batch * {o}")
+        return n_in // n
+
+    def process(self, x, out):
+        """Convolve every row of `x` (batch * signal_len samples) into `out` (batch * output_len samples); returns `out`."""
+        if isinstance(x, np.ndarray):
+            want = np.dtype(self.dtype)
+            if not isinstance(out, np.ndarray) or x.dtype != want or out.dtype != want or not x.flags.c_contiguous \
+                    or not out.flags.c_contiguous or not out.flags.writeable:
+                raise TypeError(f"FftConvolution wants contiguous {want.name} input and a writable {want.name} output")
+            batch = self._batch(x.size, out.size)
+            self._lib.check(self._lib.c.b200fft_conv_host(self._h, x.ctypes.data, out.ctypes.data, batch))
+            return out
+        import torch
+
+        tmap = {np.float32: torch.float32, np.float64: torch.float64, np.complex64: torch.complex64, np.complex128: torch.complex128}
+        want = tmap[self.dtype]
+        if not isinstance(out, torch.Tensor) or x.dtype != want or out.dtype != want or not x.is_cuda or not out.is_cuda \
+                or not x.is_contiguous() or not out.is_contiguous():
+            raise TypeError(f"FftConvolution wants contiguous CUDA tensors of {want}")
+        if x.device.index != self.device or out.device.index != self.device:
+            raise FftError(-1, f"tensors are on cuda:{x.device.index} / cuda:{out.device.index}, plan is on cuda:{self.device}")
+        batch = self._batch(x.numel(), out.numel())
+        self._lib.check(self._lib.c.b200fft_conv_device(self._h, x.data_ptr(), out.data_ptr(), batch,
+                                                        torch.cuda.current_stream(x.device).cuda_stream))
+        return out
 
 
 def shard_range(batch: int, rank: int, world: int) -> Tuple[int, int]:

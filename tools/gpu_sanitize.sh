@@ -1,5 +1,6 @@
 #!/bin/bash
-# compute-sanitizer over one small exec of every kernel family (tests/sanitize_check.py); logs summarised in $OUT/summary.txt.
+# compute-sanitizer over one small exec of every kernel family (tests/sanitize_check.py) and of every overlap-save convolution
+# variant (tests/sanitize_conv_check.py); logs summarised in $OUT/summary.txt.
 #   default build/switches: memcheck, racecheck, synccheck;  chunked two-pass (B200FFT_FUSED=0): racecheck;
 #   dataflow kernel (B200FFT_FLOW=1): memcheck;  TMA-pipelined one-pass kernels (B200FFT_PIPELINE=1): racecheck
 OUT=${1:-${TMPDIR:-/tmp}/b200fft_sanitize}
@@ -8,13 +9,18 @@ mkdir -p $OUT
 export PYTHONPATH=$PWD:$PWD/tests
 CS=/usr/local/cuda/bin/compute-sanitizer
 run() {  # name tool env...
-    local name=$1 tool=$2; shift 2
-    ( export "$@" _X=1; timeout $LIMIT $CS --tool $tool --print-limit 20 --error-exitcode 86 python tests/sanitize_check.py > $OUT/$name.log 2>&1; echo "rc=$?" >> $OUT/$name.log )
+    runs tests/sanitize_check.py "$@"
+}
+runs() {  # script name tool env...
+    local script=$1 name=$2 tool=$3; shift 3
+    ( export "$@" _X=1; timeout $LIMIT $CS --tool $tool --print-limit 20 --error-exitcode 86 python $script > $OUT/$name.log 2>&1; echo "rc=$?" >> $OUT/$name.log )
     echo "== $name: $(grep -c '^ok' $OUT/$name.log) execs ok, $(grep -E 'ERROR SUMMARY|RACECHECK SUMMARY|rc=' $OUT/$name.log | tr '\n' ' ')"
 }
 run default_memcheck memcheck
 run default_racecheck racecheck
 run default_synccheck synccheck
+runs tests/sanitize_conv_check.py conv_memcheck memcheck
+runs tests/sanitize_conv_check.py conv_racecheck racecheck
 if [ -z "$SANITIZE_DEFAULT_ONLY" ]; then
 run chunked_racecheck racecheck B200FFT_FUSED=0 SANITIZE_QUICK=1
 run flow_memcheck memcheck B200FFT_FLOW=1 SANITIZE_QUICK=1
