@@ -162,6 +162,29 @@ int b200fft_plan2d_destroy(b200fft_plan2d* plan);
 int b200fft_exec2d_device(const b200fft_plan2d* plan, const void* d_in, void* d_out, uint64_t batch, void* cuda_stream);
 int b200fft_exec2d_host(const b200fft_plan2d* plan, const void* in, void* out, uint64_t batch);
 
+/* 2-D real-input / real-output transforms of row-major [height][width] real images (a batch of them, contiguous; what
+ * numpy.fft.rfft2 / irfft2 compute over the last two axes).  forward: batch * H * W reals -> batch * H * (W/2 + 1) complex, equal
+ * to numpy.fft.rfft2(x), unnormalised, forward sign as everywhere here.  inverse: the reverse, unnormalised, so
+ * inverse(forward(x)) = H * W * x; for the spectrum of a real image it equals H * W * numpy.fft.irfft2(X, s=(H, W)).  For input
+ * that is not Hermitian-consistent it is the column inverse transforms followed by the 1-D real inverse of every row (the
+ * imaginary parts of the DC and Nyquist columns are not handled the way numpy handles them).
+ * width: even, >= 2, with W/2 any length b200fft_plan_create accepts; height: >= 1, prime factors <= 31 and at most 4096
+ * (f64: 2048); B200FFT_ERR_UNSUPPORTED otherwise.  Two passes over half-size complex data: the W/2-point complex plan over the
+ * rows, then one column pass that applies the real unpack (forward) or pack (inverse) on its load; height 1 is the 1-D real
+ * transform of length W.  Out of place only: overlapping input and output ranges are B200FFT_ERR_INVALID_ARG.  batch == 0 is a
+ * silent no-op.  Plans are immutable and thread safe; the device entry points are asynchronous on the stream and take their
+ * workspace from the stream-ordered allocator (CUDA-graph capturable). */
+typedef struct b200fft_real_plan2d b200fft_real_plan2d;
+int b200fft_real_plan2d_create(b200fft_real_plan2d** out, uint64_t height, uint64_t width, int precision, int device);
+int b200fft_real_plan2d_destroy(b200fft_real_plan2d* plan);
+/* e.g. "Real2d{62x256,rows=Direct{128}}" (rows: the W/2-point row plan's description).  Returns length or <0. */
+int b200fft_real_plan2d_describe(const b200fft_real_plan2d* plan, char* buf, uint64_t cap);
+int b200fft_real2d_forward_device(const b200fft_real_plan2d* plan, const void* d_real_in, void* d_complex_out, uint64_t batch, void* cuda_stream);
+int b200fft_real2d_inverse_device(const b200fft_real_plan2d* plan, const void* d_complex_in, void* d_real_out, uint64_t batch, void* cuda_stream);
+/* Same on host memory, synchronous (plain copies in and out, not pipelined). */
+int b200fft_real2d_forward_host(const b200fft_real_plan2d* plan, const void* real_in, void* complex_out, uint64_t batch);
+int b200fft_real2d_inverse_host(const b200fft_real_plan2d* plan, const void* complex_in, void* real_out, uint64_t batch);
+
 /* Batched FFT convolution (SURVEY 8(f).4; what scipy.signal.fftconvolve / oaconvolve do): every row of a batch of rows of
  * signal_len samples, contiguous, is convolved with ONE filter of filter_len taps fixed at plan time.  Plain sums, no scaling;
  * the result equals scipy.signal.fftconvolve(row, filter, mode):

@@ -26,8 +26,8 @@ from typing import Dict, Optional, Tuple
 
 import numpy as np
 
-__all__ = ["FftDirection", "FftPlanner", "Fft", "Library", "FftError", "Recipe", "RealFftPlanner", "RealFft", "Fft2d", "FftConvolution", "default_library",
-           "shard_range"]
+__all__ = ["FftDirection", "FftPlanner", "Fft", "Library", "FftError", "Recipe", "RealFftPlanner", "RealFft", "RealFft2d", "Fft2d", "FftConvolution",
+           "default_library", "shard_range"]
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 # B200FFT_LIB: load another build of the same C ABI (A/B measurements of kernel variants; tools/ab_two_pass.py)
@@ -130,6 +130,8 @@ class Library:
         "b200fft_plan2d_create", "b200fft_plan2d_destroy", "b200fft_exec2d_device", "b200fft_exec2d_host",
         "b200fft_conv_plan_create", "b200fft_conv_plan_destroy", "b200fft_conv_output_len", "b200fft_conv_describe",
         "b200fft_conv_device", "b200fft_conv_host",
+        "b200fft_real_plan2d_create", "b200fft_real_plan2d_destroy", "b200fft_real_plan2d_describe", "b200fft_real2d_forward_device",
+        "b200fft_real2d_inverse_device", "b200fft_real2d_forward_host", "b200fft_real2d_inverse_host",
     ]
 
     def __init__(self, path: str = DEFAULT_LIB_PATH):
@@ -180,6 +182,13 @@ class Library:
         c.b200fft_conv_describe.argtypes = [vp, ctypes.c_char_p, u64]
         c.b200fft_conv_device.argtypes = [vp, vp, vp, u64, vp]
         c.b200fft_conv_host.argtypes = [vp, vp, vp, u64]
+        c.b200fft_real_plan2d_create.argtypes = [ctypes.POINTER(vp), u64, u64, i32, i32]
+        c.b200fft_real_plan2d_destroy.argtypes = [vp]
+        c.b200fft_real_plan2d_describe.argtypes = [vp, ctypes.c_char_p, u64]
+        c.b200fft_real2d_forward_device.argtypes = [vp, vp, vp, u64, vp]
+        c.b200fft_real2d_inverse_device.argtypes = [vp, vp, vp, u64, vp]
+        c.b200fft_real2d_forward_host.argtypes = [vp, vp, vp, u64]
+        c.b200fft_real2d_inverse_host.argtypes = [vp, vp, vp, u64]
 
     def device_count(self) -> int:
         n = ctypes.c_int(0)
@@ -465,6 +474,31 @@ class Fft2d:
         return dst
 
 
+def _run_real(lib: Library, handle, precision: int, name: str, prefix: str, n: int, h: int, inverse: bool, src, dst):
+    """Type and size checks and dispatch of the real transforms (RealFft, RealFft2d): n reals <-> h complex values per transform,
+    C entry points <prefix>_{forward,inverse}_{host,device}."""
+    rdt, cdt = (np.float32, np.complex64) if precision == F32 else (np.float64, np.complex128)
+    sdt, ddt, sper, dper = (cdt, rdt, h, n) if inverse else (rdt, cdt, n, h)
+    kind = "inverse" if inverse else "forward"
+    if isinstance(src, np.ndarray):
+        if src.dtype != sdt or dst.dtype != ddt or not src.flags.c_contiguous or not dst.flags.c_contiguous or not dst.flags.writeable:
+            raise TypeError(f"{name} wants contiguous {np.dtype(sdt)} input and writable {np.dtype(ddt)} output")
+        if src.size % sper or dst.size != src.size // sper * dper:
+            raise FftError(-6, f"{name}: input holds {src.size} elements, output {dst.size}: expected batch * {sper} and batch * {dper}")
+        lib.check(getattr(lib.c, f"{prefix}_{kind}_host")(handle, src.ctypes.data, dst.ctypes.data, src.size // sper))
+        return dst
+    import torch
+
+    tmap = {np.float32: torch.float32, np.float64: torch.float64, np.complex64: torch.complex64, np.complex128: torch.complex128}
+    if src.dtype != tmap[sdt] or dst.dtype != tmap[ddt] or not src.is_cuda or not dst.is_cuda or not src.is_contiguous() or not dst.is_contiguous():
+        raise TypeError(f"{name} wants contiguous CUDA tensors of the plan's real / complex dtypes")
+    if src.numel() % sper or dst.numel() != src.numel() // sper * dper:
+        raise FftError(-6, f"{name}: input holds {src.numel()} elements, output {dst.numel()}: expected batch * {sper} and batch * {dper}")
+    lib.check(getattr(lib.c, f"{prefix}_{kind}_device")(handle, src.data_ptr(), dst.data_ptr(), src.numel() // sper,
+                                                         torch.cuda.current_stream(src.device).cuda_stream))
+    return dst
+
+
 class RealFft:
     """Real-to-complex / complex-to-real transforms of one even length (the shape of the `realfft` crate's RealToComplex /
     ComplexToReal on top of RustFFT's Fft; SURVEY 8(f).4).  forward: batch * len reals -> batch * (len/2 + 1) complex;
@@ -490,31 +524,56 @@ class RealFft:
     def complex_len(self) -> int:
         return self._len // 2 + 1
 
-    def _dtypes(self):
-        return (np.float32, np.complex64) if self._precision == F32 else (np.float64, np.complex128)
+    def _run(self, inverse: bool, src, dst):
+        return _run_real(self._lib, self._h, self._precision, "RealFft", "b200fft_real", self._len, self._len // 2 + 1, inverse, src, dst)
+
+    def forward(self, real_in, complex_out):
+        return self._run(False, real_in, complex_out)
+
+    def inverse(self, complex_in, real_out):
+        return self._run(True, complex_in, real_out)
+
+
+class RealFft2d:
+    """2-D real-to-complex / complex-to-real transforms of row-major [height][width] real images (a batch of them, contiguous), even
+    width: numpy.fft.rfft2 / irfft2 over the last two axes.  forward: batch * height * width reals -> batch * height *
+    (width/2 + 1) complex, unnormalised; inverse: the reverse, unnormalised (inverse(forward(x)) == height * width * x).  Two passes
+    over half-size complex data: the width/2-point complex plan over the rows, one column pass with the real unpack / pack fused
+    into its load.  Out of place only.  numpy arrays go through the synchronous host entry points, torch CUDA tensors through the
+    device ones (asynchronous on torch's current stream).  Immutable and safe to call from many threads."""
+
+    def __init__(self, lib: Library, height: int, width: int, precision: int, device: int):
+        self._lib, self._height, self._width, self._precision, self.device = lib, int(height), int(width), precision, device
+        self._h = ctypes.c_void_p()
+        lib.check(lib.c.b200fft_real_plan2d_create(ctypes.byref(self._h), self._height, self._width, precision, device))
+
+    def __del__(self):
+        h, self._h = getattr(self, "_h", None), None
+        if h:
+            try:
+                self._lib.c.b200fft_real_plan2d_destroy(h)
+            except Exception:
+                pass
+
+    def height(self) -> int:
+        return self._height
+
+    def width(self) -> int:
+        return self._width
+
+    def complex_width(self) -> int:
+        return self._width // 2 + 1
+
+    def describe(self) -> str:
+        buf = ctypes.create_string_buffer(512)
+        rc = self._lib.c.b200fft_real_plan2d_describe(self._h, buf, len(buf))
+        if rc < 0:
+            self._lib.check(rc)
+        return buf.value.decode()
 
     def _run(self, inverse: bool, src, dst):
-        rdt, cdt = self._dtypes()
-        n, h = self._len, self._len // 2 + 1
-        sdt, ddt, sper, dper = (cdt, rdt, h, n) if inverse else (rdt, cdt, n, h)
-        if isinstance(src, np.ndarray):
-            if src.dtype != sdt or dst.dtype != ddt or not src.flags.c_contiguous or not dst.flags.c_contiguous or not dst.flags.writeable:
-                raise TypeError(f"RealFft wants contiguous {np.dtype(sdt)} input and writable {np.dtype(ddt)} output")
-            if src.size % sper or dst.size != src.size // sper * dper:
-                raise FftError(-6, f"RealFft: input holds {src.size} elements, output {dst.size}: expected batch * {sper} and batch * {dper}")
-            fn = self._lib.c.b200fft_real_inverse_host if inverse else self._lib.c.b200fft_real_forward_host
-            self._lib.check(fn(self._h, src.ctypes.data, dst.ctypes.data, src.size // sper))
-            return dst
-        import torch
-
-        tmap = {np.float32: torch.float32, np.float64: torch.float64, np.complex64: torch.complex64, np.complex128: torch.complex128}
-        if src.dtype != tmap[sdt] or dst.dtype != tmap[ddt] or not src.is_cuda or not dst.is_cuda or not src.is_contiguous() or not dst.is_contiguous():
-            raise TypeError("RealFft wants contiguous CUDA tensors of the plan's real / complex dtypes")
-        if src.numel() % sper or dst.numel() != src.numel() // sper * dper:
-            raise FftError(-6, f"RealFft: input holds {src.numel()} elements, output {dst.numel()}: expected batch * {sper} and batch * {dper}")
-        fn = self._lib.c.b200fft_real_inverse_device if inverse else self._lib.c.b200fft_real_forward_device
-        self._lib.check(fn(self._h, src.data_ptr(), dst.data_ptr(), src.numel() // sper, torch.cuda.current_stream(src.device).cuda_stream))
-        return dst
+        return _run_real(self._lib, self._h, self._precision, "RealFft2d", "b200fft_real2d", self._height * self._width,
+                         self._height * self.complex_width(), inverse, src, dst)
 
     def forward(self, real_in, complex_out):
         return self._run(False, real_in, complex_out)
@@ -539,6 +598,7 @@ class RealFftPlanner:
             raise FftError(-2, "no sm_90 CUDA device is visible (there is no CPU fallback)")
         self.device = device
         self._cache: Dict[int, RealFft] = {}
+        self._cache_2d: Dict[Tuple[int, int], RealFft2d] = {}
         self._lock = threading.Lock()
 
     def plan_fft(self, len: int) -> RealFft:
@@ -546,6 +606,15 @@ class RealFftPlanner:
             f = self._cache.get(int(len))
             if f is None:
                 f = self._cache[int(len)] = RealFft(self._lib, int(len), self._precision, self.device)
+            return f
+
+    def plan_fft_2d(self, height: int, width: int) -> RealFft2d:
+        """2-D real transform of [height][width] images (even width), cached per shape; see RealFft2d."""
+        key = (int(height), int(width))
+        with self._lock:
+            f = self._cache_2d.get(key)
+            if f is None:
+                f = self._cache_2d[key] = RealFft2d(self._lib, key[0], key[1], self._precision, self.device)
             return f
 
     def plan_convolution(self, filter, signal_len: int, mode: str = "full") -> FftConvolution:

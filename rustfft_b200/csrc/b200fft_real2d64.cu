@@ -1,0 +1,4 @@
+// libb200fft.so -- the f64 column passes of the 2-D real transforms (Real2dColumnKernel, kernels.h), in a translation unit of their own.
+#include "rt_cuda.h"
+#define B2_PART_REAL2D64 1
+#include "impl.inl"

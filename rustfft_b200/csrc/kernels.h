@@ -729,16 +729,34 @@ struct SmoothKernel {
 //                    [k1][n2], each entry rounded once); the N2-point result k2 goes to out[b*N + k2*N1 + k1].
 //                    Threads: element fastest (contiguous loads) until the last stage, row fastest there
 //                    (adjacent rows are adjacent in the output); shared memory [row][odd pitch].
+// The body is SmoothPassBody; SmoothPassKernel is its R2D = 0 form, unchanged.  R2D (MODE 1 only, a compile-time variant that
+// Real2dColumnKernel names) is the column pass of the 2-D real transforms, with the per-row real unpack / pack of real.h
+// (M = W / 2) applied on the load:
+//   R2D 1 (forward):  M + 1 output columns k of an [H][M + 1] spectrum from Z = the M-point row FFTs [H][M] of the real image:
+//                     element e = E + W_W^k O, E = (Z[e][k mod M] + conj Z[e][(M-k) mod M]) / 2, O = (... - ...) / 2i
+//   R2D 2 (inverse):  M output columns k of Z' [H][M] from the [H][M + 1] spectrum X, the row index of the partner reflected
+//                     (IFFT_H of conj X[-k1][.] is conj of IFFT_H of X[k1][.]):
+//                     element k1 = A + i conj(W_W^k) B, A / B = X[k1][k] +/- conj X[(H-k1) mod H][M-k]
+// Column slot c of the `other` slots of an image holds column c / 2 (c even) or other - 1 - c / 2 (c odd), so the two columns a
+// thread's load gathers are one warp's two contiguous runs, and lanes 2i and 2i + 1 read the same lines.  Store: [H][other].
 // ------------------------------------------------------------------------------------------
-template <typename T, bool SW, int MODE, int RMAX = 31>
-struct SmoothPassKernel {
+template <typename T>
+struct Real2dPassArgs {
+    const cx<T>* wk;    // W_W^k, k = 0 .. M
+    uint32_t half_w;    // M = W / 2
+    uint32_t in_pitch;  // complex elements per input row: M (forward), M + 1 (inverse)
+};
+struct NoPassArgs {};
+template <typename T, bool SW, int MODE, int RMAX, int R2D>
+struct SmoothPassBody {
+    static_assert(R2D == 0 || (MODE == 1 && SW == (R2D == 2)), "the 2-D real column passes are MODE 1; the inverse one runs swapped");
     using T_ = T;
     static constexpr int NT = 256;
     static constexpr int MIN_BLOCKS = RMAX > 16 ? 2 : 3;
     static constexpr int MAX_STAGES = 8;
     static constexpr int NPHASE = MAX_STAGES;
     static constexpr size_t SMEM_BYTES = 0;  // run-time sized: Params::smem_bytes
-    struct Params {
+    struct Params : std::conditional_t<R2D != 0, Real2dPassArgs<T>, NoPassArgs> {
         const cx<T>* in;
         cx<T>* out;
         const cx<T>* tw;       // packed stage twiddles of this pass' length (layout as in SmoothKernel)
@@ -781,6 +799,39 @@ struct SmoothPassKernel {
         return MODE == 1 ? (size_t)e * p.f_per_cta + f : (size_t)f * p.pitch + e;
     }
 
+    // 2-D real passes: the column a slot holds (partners adjacent, see above)
+    static B2_HD uint32_t real2d_column(const Params& p, uint32_t c) { return (c & 1u) ? p.other - 1u - (c >> 1) : c >> 1; }
+    // the R elements e = i + q T_s of column k of image b, unpacked (R2D 1) or packed (R2D 2) on the load -- real.h's arithmetic
+    template <int R>
+    static B2_HD void real2d_load(const Params& p, uint32_t b, uint32_t k, uint32_t i, uint32_t T_s, cx<T>* a) {
+        const uint32_t M = p.half_w, H = p.n;
+        const cx<T>* src = p.in + (uint64_t)b * H * p.in_pitch;
+        if constexpr (R2D == 1) {
+            const uint32_t ka = k == M ? 0u : k, kb = k == 0 ? 0u : M - k;
+            const cx<T> w = ldg(p.wk + k);
+            const T half = (T)0.5;
+            B2_UNROLL
+            for (int q = 0; q < R; ++q) {
+                const cx<T>* row = src + (uint64_t)(i + (uint32_t)q * T_s) * M;
+                const cx<T> zk = ldg(row + ka), zm = conj(ldg(row + kb));
+                const cx<T> e = mk<T>((zk.x + zm.x) * half, (zk.y + zm.y) * half);
+                const cx<T> d = mk<T>((zk.x - zm.x) * half, (zk.y - zm.y) * half);  // = i O
+                const cx<T> o = mk<T>(d.y, -d.x);                                     // O = d / i
+                a[q] = e + cmul(o, w);
+            }
+        } else {
+            const uint32_t P = p.in_pitch;  // M + 1
+            const cx<T> w = conj(ldg(p.wk + k));
+            B2_UNROLL
+            for (int q = 0; q < R; ++q) {
+                const uint32_t e = i + (uint32_t)q * T_s, er = e == 0 ? 0u : H - e;
+                const cx<T> xk = ldg(src + (uint64_t)e * P + k), xm = conj(ldg(src + (uint64_t)er * P + (M - k)));
+                const cx<T> s = xk + xm, t = cmul(xk - xm, w);  // A, conj(W^k) B
+                a[q] = swap_ri(s + mk<T>(-t.y, t.x));           // A + i conj(W^k) B, swapped for the inverse FFT
+            }
+        }
+    }
+
     template <int R>
     static B2_HD void stage(const Params& p, uint32_t bid, int tid, int s, cx<T>* smem) {
         const uint32_t F = p.f_per_cta;
@@ -807,7 +858,9 @@ struct SmoothPassKernel {
             const uint32_t k = i - p.div_p[s].div(i) * pp;
             cx<T> a[R];
             if (first) {
-                if (MODE == 1 && p.gt) {
+                if constexpr (R2D != 0) {
+                    real2d_load<R>(p, b, real2d_column(p, c), i, T_s, a);
+                } else if (MODE == 1 && p.gt) {
                     const cx<T>* src = p.in + (uint64_t)b * p.NN;
                     const uint32_t o2 = ldg_u32(p.crt2 + c);
                     B2_UNROLL
@@ -890,7 +943,9 @@ struct SmoothPassKernel {
                     }
                 }
             } else if (last) {
-                cx<T>* dst = p.out + (uint64_t)b * p.NN + c;
+                cx<T>* dst;
+                if constexpr (R2D != 0) dst = p.out + (uint64_t)b * p.NN + real2d_column(p, c);
+                else dst = p.out + (uint64_t)b * p.NN + c;
                 B2_UNROLL
                 for (int m = 0; m < R; ++m) {
                     const cx<T> v = ((MODE == 2 && SW) || (MODE == 1 && p.swap_out)) ? swap_ri(a[m]) : a[m];
@@ -926,6 +981,11 @@ struct SmoothPassKernel {
         }
     }
 };
+template <typename T, bool SW, int MODE, int RMAX = 31>
+struct SmoothPassKernel : SmoothPassBody<T, SW, MODE, RMAX, 0> {};
+// R2D 1: forward (unpack, then the forward column FFT);  R2D 2: inverse (pack, then the inverse column FFT, re/im swapped)
+template <typename T, int R2D, int RMAX>
+struct Real2dColumnKernel : SmoothPassBody<T, R2D == 2, 1, RMAX, R2D> {};
 
 // ------------------------------------------------------------------------------------------
 // SmoothConvKernel: a whole convolution-based transform in ONE CTA pass over a SMOOTH inner length M (prime factors
