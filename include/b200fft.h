@@ -212,6 +212,35 @@ int b200fft_conv_device(const b200fft_conv_plan* plan, const void* d_in, void* d
 /* Same on host memory, synchronous (plain copies in and out, not pipelined). */
 int b200fft_conv_host(const b200fft_conv_plan* plan, const void* in, void* out, uint64_t batch);
 
+/* Batched 2-D FFT convolution of real images: every [height][width] image of a batch of real images (row-major, contiguous) is
+ * convolved with ONE real filter of [filter_height][filter_width] taps (row-major, host memory) fixed at plan time.  Plain sums,
+ * no scaling; the result equals scipy.signal.fftconvolve(image, filter, mode) in 2-D, with the B200FFT_CONV_* modes per axis:
+ *   FULL   (H + kh - 1) x (W + kw - 1) outputs
+ *   SAME   H x W outputs starting at full index ((kh - 1) / 2, (kw - 1) / 2) (scipy's centring, also for a filter larger than the image)
+ *   VALID  (H - kh + 1) x (W - kw + 1) outputs starting at full index (kh - 1, kw - 1); needs H >= kh and W >= kw (the inputs are
+ *          not swapped as scipy does)
+ * Cross-correlation of an image with h is the convolution with h[::-1, ::-1] (the filter reversed along both axes).
+ * Any H, W, kh, kw >= 1, odd widths included.  The plan runs a circular convolution of P x Q, Q = 2 M, with P >= H + kh - 1 - r0
+ * and Q >= W + kw - 1 - c0 ((r0, c0) = the first output's full index), which leaves every output alias-free; P and M are the
+ * smallest 7-smooth numbers >= those bounds (and >= 2) and must be at most 4096 (f64: 2048), B200FFT_ERR_UNSUPPORTED otherwise.
+ * Three passes over half-size complex data: M-point row FFTs of the images, one column pass (real unpack, P-point FFT, product
+ * with the filter's spectrum, inverse P-point FFT, only the output rows stored), inverse M-point row FFTs with the real pack that
+ * store only the output columns.  Out of place only: overlapping input and output ranges are B200FFT_ERR_INVALID_ARG.
+ * batch == 0 is a silent no-op.  Plans are immutable and thread safe; the device entry point is asynchronous on the stream and
+ * takes its two workspaces from the stream-ordered allocator (CUDA-graph capturable). */
+typedef struct b200fft_conv2d_plan b200fft_conv2d_plan;
+int b200fft_conv2d_plan_create(b200fft_conv2d_plan** out, uint64_t height, uint64_t width, const void* filter, uint64_t filter_height,
+                               uint64_t filter_width, int mode, int precision, int device);
+int b200fft_conv2d_plan_destroy(b200fft_conv2d_plan* plan);
+/* Output image shape: *out_height x *out_width per input image.  Returns status. */
+int b200fft_conv2d_output_shape(const b200fft_conv2d_plan* plan, uint64_t* out_height, uint64_t* out_width);
+/* e.g. "Conv2d{1080x1920,k=31x31,full,pad=1120x1960}" (pad = P x Q).  Returns length or <0. */
+int b200fft_conv2d_describe(const b200fft_conv2d_plan* plan, char* buf, uint64_t cap);
+/* d_in: batch * H * W reals, d_out: batch * Ho * Wo reals on the plan's device; asynchronous on `cuda_stream`. */
+int b200fft_conv2d_device(const b200fft_conv2d_plan* plan, const void* d_in, void* d_out, uint64_t batch, void* cuda_stream);
+/* Same on host memory, synchronous (plain copies in and out, not pipelined). */
+int b200fft_conv2d_host(const b200fft_conv2d_plan* plan, const void* in, void* out, uint64_t batch);
+
 /* Message of the last failing call on this thread ("" if none). */
 const char* b200fft_last_error(void);
 /* Library build string: "b200fft <version> sm_90a" */

@@ -27,6 +27,7 @@ from typing import Dict, Optional, Tuple
 import numpy as np
 
 __all__ = ["FftDirection", "FftPlanner", "Fft", "Library", "FftError", "Recipe", "RealFftPlanner", "RealFft", "RealFft2d", "Fft2d", "FftConvolution",
+           "FftConvolution2d",
            "default_library", "shard_range"]
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -132,6 +133,8 @@ class Library:
         "b200fft_conv_device", "b200fft_conv_host",
         "b200fft_real_plan2d_create", "b200fft_real_plan2d_destroy", "b200fft_real_plan2d_describe", "b200fft_real2d_forward_device",
         "b200fft_real2d_inverse_device", "b200fft_real2d_forward_host", "b200fft_real2d_inverse_host",
+        "b200fft_conv2d_plan_create", "b200fft_conv2d_plan_destroy", "b200fft_conv2d_output_shape", "b200fft_conv2d_describe",
+        "b200fft_conv2d_device", "b200fft_conv2d_host",
     ]
 
     def __init__(self, path: str = DEFAULT_LIB_PATH):
@@ -189,6 +192,12 @@ class Library:
         c.b200fft_real2d_inverse_device.argtypes = [vp, vp, vp, u64, vp]
         c.b200fft_real2d_forward_host.argtypes = [vp, vp, vp, u64]
         c.b200fft_real2d_inverse_host.argtypes = [vp, vp, vp, u64]
+        c.b200fft_conv2d_plan_create.argtypes = [ctypes.POINTER(vp), u64, u64, vp, u64, u64, i32, i32, i32]
+        c.b200fft_conv2d_plan_destroy.argtypes = [vp]
+        c.b200fft_conv2d_output_shape.argtypes = [vp, ctypes.POINTER(u64), ctypes.POINTER(u64)]
+        c.b200fft_conv2d_describe.argtypes = [vp, ctypes.c_char_p, u64]
+        c.b200fft_conv2d_device.argtypes = [vp, vp, vp, u64, vp]
+        c.b200fft_conv2d_host.argtypes = [vp, vp, vp, u64]
 
     def device_count(self) -> int:
         n = ctypes.c_int(0)
@@ -622,6 +631,11 @@ class RealFftPlanner:
         cached: the filter is data)."""
         return FftConvolution(self._lib, filter, signal_len, mode, True, self._precision, self.device)
 
+    def plan_convolution_2d(self, filter, image_shape, mode: str = "full") -> "FftConvolution2d":
+        """2-D convolution of real images of image_shape = (height, width) with the real 2-D `filter`; see FftConvolution2d (not
+        cached: the filter is data)."""
+        return FftConvolution2d(self._lib, filter, image_shape, mode, self._precision, self.device)
+
 
 class FftConvolution:
     """Batched FFT convolution with one filter fixed at plan time: every contiguous row of signal_len samples becomes
@@ -708,6 +722,95 @@ class FftConvolution:
         batch = self._batch(x.numel(), out.numel())
         self._lib.check(self._lib.c.b200fft_conv_device(self._h, x.data_ptr(), out.data_ptr(), batch,
                                                         torch.cuda.current_stream(x.device).cuda_stream))
+        return out
+
+
+class FftConvolution2d:
+    """Batched 2-D FFT convolution of real images with one real filter fixed at plan time: every contiguous [height][width] image
+    becomes scipy.signal.fftconvolve(image, filter, mode) -- plain sums, no scaling.  mode "full" ((height + kh - 1) x
+    (width + kw - 1) outputs), "same" (height x width, scipy's centring) or "valid" ((height - kh + 1) x (width - kw + 1), needs an
+    image at least as large as the filter; the inputs are not swapped).  Cross-correlation with h is the convolution with
+    h[::-1, ::-1].
+
+    Three passes over half-size complex data (row FFTs, one fused column pass with the filter's spectrum, inverse row FFTs that
+    store only the requested pixels), out of place only.  The padded size of the circular convolution must stay within 4096 rows
+    and 4096 complex columns (f64: 2048).  numpy arrays go through the synchronous host entry point, torch CUDA tensors through the
+    device one (asynchronous on torch's current stream).  Immutable and safe to call from many threads."""
+
+    MODES = FftConvolution.MODES
+
+    def __init__(self, lib: Library, filter, image_shape, mode: str, precision: int, device: int):
+        if mode not in self.MODES:
+            raise FftError(-1, f"unknown convolution mode {mode!r}: expected one of {sorted(self.MODES)}")
+        self._lib, self._precision, self.device, self.mode = lib, precision, device, mode
+        self._shape = tuple(int(v) for v in image_shape)
+        if len(self._shape) != 2:
+            raise TypeError("image_shape must be (height, width)")
+        if np.iscomplexobj(filter):
+            raise TypeError("a real convolution plan needs a real filter")
+        h = np.ascontiguousarray(np.asarray(filter), dtype=self.dtype)
+        if h.ndim != 2:
+            raise TypeError("the filter must be 2-D")
+        self._h = ctypes.c_void_p()
+        lib.check(lib.c.b200fft_conv2d_plan_create(ctypes.byref(self._h), self._shape[0], self._shape[1], h.ctypes.data, h.shape[0],
+                                                   h.shape[1], self.MODES[mode], precision, device))
+        ho, wo = ctypes.c_uint64(), ctypes.c_uint64()
+        lib.check(lib.c.b200fft_conv2d_output_shape(self._h, ctypes.byref(ho), ctypes.byref(wo)))
+        self._out_shape = (int(ho.value), int(wo.value))
+
+    def __del__(self):
+        h, self._h = getattr(self, "_h", None), None
+        if h:
+            try:
+                self._lib.c.b200fft_conv2d_plan_destroy(h)
+            except Exception:
+                pass
+
+    @property
+    def dtype(self):
+        return np.float32 if self._precision == F32 else np.float64
+
+    def image_shape(self) -> Tuple[int, int]:
+        return self._shape
+
+    def output_shape(self) -> Tuple[int, int]:
+        return self._out_shape
+
+    def describe(self) -> str:
+        buf = ctypes.create_string_buffer(256)
+        rc = self._lib.c.b200fft_conv2d_describe(self._h, buf, len(buf))
+        if rc < 0:
+            self._lib.check(rc)
+        return buf.value.decode()
+
+    def _batch(self, n_in: int, n_out: int) -> int:
+        n, o = self._shape[0] * self._shape[1], self._out_shape[0] * self._out_shape[1]
+        if n_in % n or n_out != n_in // n * o:
+            raise FftError(-6, f"FftConvolution2d: input holds {n_in} samples, output {n_out}: expected batch * {n} and batch * {o}")
+        return n_in // n
+
+    def process(self, x, out):
+        """Convolve every image of `x` (batch * height * width samples, any shape) into `out` (batch * output height * output width
+        samples); returns `out`."""
+        if isinstance(x, np.ndarray):
+            want = np.dtype(self.dtype)
+            if not isinstance(out, np.ndarray) or x.dtype != want or out.dtype != want or not x.flags.c_contiguous \
+                    or not out.flags.c_contiguous or not out.flags.writeable:
+                raise TypeError(f"FftConvolution2d wants contiguous {want.name} input and a writable {want.name} output")
+            batch = self._batch(x.size, out.size)
+            self._lib.check(self._lib.c.b200fft_conv2d_host(self._h, x.ctypes.data, out.ctypes.data, batch))
+            return out
+        import torch
+
+        want = torch.float32 if self._precision == F32 else torch.float64
+        if not isinstance(out, torch.Tensor) or x.dtype != want or out.dtype != want or not x.is_cuda or not out.is_cuda \
+                or not x.is_contiguous() or not out.is_contiguous():
+            raise TypeError(f"FftConvolution2d wants contiguous CUDA tensors of {want}")
+        if x.device.index != self.device or out.device.index != self.device:
+            raise FftError(-1, f"tensors are on cuda:{x.device.index} / cuda:{out.device.index}, plan is on cuda:{self.device}")
+        batch = self._batch(x.numel(), out.numel())
+        self._lib.check(self._lib.c.b200fft_conv2d_device(self._h, x.data_ptr(), out.data_ptr(), batch,
+                                                          torch.cuda.current_stream(x.device).cuda_stream))
         return out
 
 
