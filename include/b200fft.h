@@ -142,7 +142,8 @@ int b200fft_exec_device_ws(const b200fft_plan* plan, const void* d_in, void* d_o
 
 /* Real-input / real-output transforms of even length on top of the complex plans (SURVEY 8(f).4: what the `realfft` crate adds above
  * RustFFT's Fft trait; RustFFT itself has none).  forward: batch * len reals -> batch * (len/2 + 1) complex (the non-redundant half of the
- * spectrum); inverse: the reverse, unnormalised (inverse(forward(x)) = len * x).  Device-resident entry points (asynchronous on the stream)
+ * spectrum); inverse: the reverse, unnormalised (inverse(forward(x)) = len * x), equal to len * numpy.fft.irfft(X, len) for any X: the
+ * imaginary parts of X[0] and X[len/2] are ignored, as numpy ignores them.  Device-resident entry points (asynchronous on the stream)
  * and synchronous host ones (plain copies in and out, not pipelined). */
 typedef struct b200fft_real_plan b200fft_real_plan;
 int b200fft_real_plan_create(b200fft_real_plan** out, uint64_t len, int precision, int device);
@@ -165,9 +166,9 @@ int b200fft_exec2d_host(const b200fft_plan2d* plan, const void* in, void* out, u
 /* 2-D real-input / real-output transforms of row-major [height][width] real images (a batch of them, contiguous; what
  * numpy.fft.rfft2 / irfft2 compute over the last two axes).  forward: batch * H * W reals -> batch * H * (W/2 + 1) complex, equal
  * to numpy.fft.rfft2(x), unnormalised, forward sign as everywhere here.  inverse: the reverse, unnormalised, so
- * inverse(forward(x)) = H * W * x; for the spectrum of a real image it equals H * W * numpy.fft.irfft2(X, s=(H, W)).  For input
- * that is not Hermitian-consistent it is the column inverse transforms followed by the 1-D real inverse of every row (the
- * imaginary parts of the DC and Nyquist columns are not handled the way numpy handles them).
+ * inverse(forward(x)) = H * W * x.  For any half spectrum X it equals H * W * numpy.fft.irfft2(X, s=(H, W)): the inverse column
+ * transforms, then numpy's irfft of every row, which keeps only the real parts of the DC and Nyquist entries.  So of columns 0 and
+ * W/2 only the Hermitian parts (X[k1][k] + conj X[-k1][k]) / 2 count; the rest cannot be represented by a real image.
  * width: even, >= 2, with W/2 any length b200fft_plan_create accepts; height: >= 1, prime factors <= 31 and at most 4096
  * (f64: 2048); B200FFT_ERR_UNSUPPORTED otherwise.  Two passes over half-size complex data: the W/2-point complex plan over the
  * rows, then one column pass that applies the real unpack (forward) or pack (inverse) on its load; height 1 is the 1-D real

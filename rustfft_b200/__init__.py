@@ -511,7 +511,8 @@ def _run_real(lib: Library, handle, precision: int, name: str, prefix: str, n: i
 class RealFft:
     """Real-to-complex / complex-to-real transforms of one even length (the shape of the `realfft` crate's RealToComplex /
     ComplexToReal on top of RustFFT's Fft; SURVEY 8(f).4).  forward: batch * len reals -> batch * (len/2 + 1) complex;
-    inverse: the reverse, unnormalised (inverse(forward(x)) == len * x).  numpy arrays go through the synchronous host entry
+    inverse: the reverse, unnormalised (inverse(forward(x)) == len * x), equal to len * numpy.fft.irfft(X, len) for any X: the
+    imaginary parts of X[0] and X[len/2] are ignored, as numpy ignores them.  numpy arrays go through the synchronous host entry
     points, torch CUDA tensors through the device ones (asynchronous on torch's current stream)."""
 
     def __init__(self, lib: Library, length: int, precision: int, device: int):
@@ -546,7 +547,9 @@ class RealFft:
 class RealFft2d:
     """2-D real-to-complex / complex-to-real transforms of row-major [height][width] real images (a batch of them, contiguous), even
     width: numpy.fft.rfft2 / irfft2 over the last two axes.  forward: batch * height * width reals -> batch * height *
-    (width/2 + 1) complex, unnormalised; inverse: the reverse, unnormalised (inverse(forward(x)) == height * width * x).  Two passes
+    (width/2 + 1) complex, unnormalised; inverse: the reverse, unnormalised (inverse(forward(x)) == height * width * x), equal to
+    height * width * numpy.fft.irfft2(X, s=(height, width)) for any half spectrum X (of columns 0 and width/2 only the Hermitian
+    parts count, as in numpy).  Two passes
     over half-size complex data: the width/2-point complex plan over the rows, one column pass with the real unpack / pack fused
     into its load.  Out of place only.  numpy arrays go through the synchronous host entry points, torch CUDA tensors through the
     device ones (asynchronous on torch's current stream).  Immutable and safe to call from many threads."""

@@ -737,6 +737,8 @@ struct SmoothKernel {
 //   R2D 2 (inverse):  M output columns k of Z' [H][M] from the [H][M + 1] spectrum X, the row index of the partner reflected
 //                     (IFFT_H of conj X[-k1][.] is conj of IFFT_H of X[k1][.]):
 //                     element k1 = A + i conj(W_W^k) B, A / B = X[k1][k] +/- conj X[(H-k1) mod H][M-k]
+//   R2D 3 (inverse, column 0 again; Real2dDcColumnKernel): the same element from the Hermitian parts of columns 0 and M, as
+//                     numpy.fft.irfft2 keeps them; it overwrites the R2D 2 pass's column 0
 // Column slot c of the `other` slots of an image holds column c / 2 (c even) or other - 1 - c / 2 (c odd), so the two columns a
 // thread's load gathers are one warp's two contiguous runs, and lanes 2i and 2i + 1 read the same lines.  Store: [H][other].
 // ------------------------------------------------------------------------------------------
@@ -749,7 +751,7 @@ struct Real2dPassArgs {
 struct NoPassArgs {};
 template <typename T, bool SW, int MODE, int RMAX, int R2D>
 struct SmoothPassBody {
-    static_assert(R2D == 0 || (MODE == 1 && SW == (R2D == 2)), "the 2-D real column passes are MODE 1; the inverse one runs swapped");
+    static_assert(R2D == 0 || (MODE == 1 && SW == (R2D >= 2)), "the 2-D real column passes are MODE 1; the inverse ones run swapped");
     using T_ = T;
     static constexpr int NT = 256;
     static constexpr int MIN_BLOCKS = RMAX > 16 ? 2 : 3;
@@ -799,6 +801,11 @@ struct SmoothPassBody {
         return MODE == 1 ? (size_t)e * p.f_per_cta + f : (size_t)f * p.pitch + e;
     }
 
+    // elements between the output rows: `other`, except R2D 3 (one slot per image, column 0 of rows of M)
+    static B2_HD uint32_t out_pitch(const Params& p) {
+        if constexpr (R2D == 3) return p.half_w;
+        else return p.other;
+    }
     // 2-D real passes: the column a slot holds (partners adjacent, see above)
     static B2_HD uint32_t real2d_column(const Params& p, uint32_t c) { return (c & 1u) ? p.other - 1u - (c >> 1) : c >> 1; }
     // the R elements e = i + q T_s of column k of image b, unpacked (R2D 1) or packed (R2D 2) on the load -- real.h's arithmetic
@@ -818,6 +825,21 @@ struct SmoothPassBody {
                 const cx<T> d = mk<T>((zk.x - zm.x) * half, (zk.y - zm.y) * half);  // = i O
                 const cx<T> o = mk<T>(d.y, -d.x);                                     // O = d / i
                 a[q] = e + cmul(o, w);
+            }
+        } else if constexpr (R2D == 3) {
+            // column 0 only (k = 0, W^0 = 1): the Hermitian parts (X[k1][0] + conj X[-k1][0]) / 2 and (X[-k1][M] + conj X[k1][M]) / 2,
+            // then A + i B as above; equal to the R2D 2 element, bit for bit, when columns 0 and M are Hermitian
+            const uint32_t P = p.in_pitch;  // M + 1
+            const T half = (T)0.5;
+            (void)k;
+            B2_UNROLL
+            for (int q = 0; q < R; ++q) {
+                const uint32_t e = i + (uint32_t)q * T_s, er = e == 0 ? 0u : H - e;
+                const cx<T> x0 = ldg(src + (uint64_t)e * P), xr = conj(ldg(src + (uint64_t)er * P));
+                const cx<T> xm = conj(ldg(src + (uint64_t)er * P + M)), xn = ldg(src + (uint64_t)e * P + M);
+                const cx<T> xk = mk<T>((x0.x + xr.x) * half, (x0.y + xr.y) * half), xh = mk<T>((xm.x + xn.x) * half, (xm.y + xn.y) * half);
+                const cx<T> s = xk + xh, t = xk - xh;
+                a[q] = swap_ri(s + mk<T>(-t.y, t.x));
             }
         } else {
             const uint32_t P = p.in_pitch;  // M + 1
@@ -949,7 +971,7 @@ struct SmoothPassBody {
                 B2_UNROLL
                 for (int m = 0; m < R; ++m) {
                     const cx<T> v = ((MODE == 2 && SW) || (MODE == 1 && p.swap_out)) ? swap_ri(a[m]) : a[m];
-                    cx<T>* d = dst + (uint64_t)(base + (uint32_t)m * pp) * p.other;
+                    cx<T>* d = dst + (uint64_t)(base + (uint32_t)m * pp) * out_pitch(p);
                     if (MODE == 2) st_cs(d, v); else *d = v;  // pass A's output is re-read from L2 by pass B
                 }
             } else {
@@ -986,6 +1008,10 @@ struct SmoothPassKernel : SmoothPassBody<T, SW, MODE, RMAX, 0> {};
 // R2D 1: forward (unpack, then the forward column FFT);  R2D 2: inverse (pack, then the inverse column FFT, re/im swapped)
 template <typename T, int R2D, int RMAX>
 struct Real2dColumnKernel : SmoothPassBody<T, R2D == 2, 1, RMAX, R2D> {};
+// R2D 3: the inverse column pass again, for column 0 alone, after Real2dColumnKernel<T, 2>: numpy.fft.irfft2's last-axis irfft keeps
+// only the Hermitian parts of columns 0 and M, which the plain pack does not separate.  One slot (column 0) per image.
+template <typename T, int RMAX>
+struct Real2dDcColumnKernel : SmoothPassBody<T, true, 1, RMAX, 3> {};
 
 // ------------------------------------------------------------------------------------------
 // SmoothConvKernel: a whole convolution-based transform in ONE CTA pass over a SMOOTH inner length M (prime factors

@@ -4,7 +4,8 @@
 //     E[k] = (Z[k] + conj Z[M-k]) / 2,   O[k] = (Z[k] - conj Z[M-k]) / (2i)        (FFTs of the even / odd samples)
 //     X[k] = E[k] + W_N^k O[k],          X[M-k] = conj(E[k] - W_N^k O[k]),          k = 0 .. M/2   (X has M + 1 entries)
 // The inverse packs the M + 1 spectrum entries back (scaled by 2, so that c2r(r2c(x)) = N x -- unnormalised like everything else here
-// and like the realfft crate) and runs the M-point inverse plan straight into the real output.
+// and like the realfft crate) and runs the M-point inverse plan straight into the real output.  Like numpy.fft.irfft it reads only
+// the real parts of X[0] and X[M]: their imaginary parts have no real signal to belong to.
 // One elementwise pass each, one thread per pair (k, M - k).
 #pragma once
 #include "kernels.h"
@@ -48,7 +49,11 @@ struct RealPackKernel {
         } else {
             const cx<T>* x = p.in + (uint64_t)b * (M + 1);
             cx<T>* z = p.out + (uint64_t)b * M;
-            const cx<T> xk = x[k], xm = conj(x[km]);
+            cx<T> xk = x[k], xm = conj(x[km]);
+            if (k == 0) {  // numpy's irfft: a real output has no room for Im X[0] or Im X[M], so both are dropped
+                xk.y = (T)0;
+                xm.y = (T)0;
+            }
             const cx<T> a = xk + xm, bb = xk - xm;
             const cx<T> t = cmul(bb, conj(w));   // conj(W^k) B
             const cx<T> it = mk<T>(-t.y, t.x);   // i conj(W^k) B

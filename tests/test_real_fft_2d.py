@@ -172,6 +172,20 @@ def test_real2d_column_kernels_spills():
     assert got == SPILL_STORES
 
 
+# the inverse's second pass over column 0 alone (numpy's irfft2 semantics), keyed (precision, largest radix): f32 spill-free
+DC_SPILL_STORES = {("f", 16): 0, ("f", 31): 0, ("d", 16): 576, ("d", 31): 15136}
+_DC_ENTRY = re.compile(
+    r"Compiling entry function '_ZN2b214run_kernel_dynINS_20Real2dDcColumnKernelI([fd])Li(\d+)EEEEEvNT_6ParamsE' for 'sm_90a'\n"
+    r"(?:ptxas info\s*: Function properties for \S+\n)?\s*(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads\n")
+
+
+def test_real2d_dc_column_kernels_spills():
+    if not os.path.exists(PTXAS_LOG):
+        pytest.fail(f"{PTXAS_LOG} missing: build() writes it")
+    got = {(t, int(rmax)): int(st) for t, rmax, _, st, _ in _DC_ENTRY.findall(open(PTXAS_LOG).read())}
+    assert got == DC_SPILL_STORES
+
+
 # ---- GPU ------------------------------------------------------------------------------------------------------------------------
 @pytest.mark.gpu
 @pytest.mark.parametrize("case", GPU_CASES, ids=case_id)
