@@ -242,6 +242,33 @@ int b200fft_conv2d_device(const b200fft_conv2d_plan* plan, const void* d_in, voi
 /* Same on host memory, synchronous (plain copies in and out, not pipelined). */
 int b200fft_conv2d_host(const b200fft_conv2d_plan* plan, const void* in, void* out, uint64_t batch);
 
+/* Batched real-to-real transforms: DCTs and DSTs of types II, III and IV (what the `rustdct` crate's Dct2 / Dct3 / Dct4 / Dst2 / Dst3
+ * / Dst4 traits add above RustFFT's Fft).  A buffer holds batch * len reals (float / double), contiguous rows; d_in == d_out (in
+ * place) is allowed, any other overlap of the input and output ranges is B200FFT_ERR_INVALID_ARG.  Unnormalised; for a row x and
+ * n, k in 0 .. len - 1 (N = len):
+ *   DCT2  X[k] = sum x[n] cos(pi (2n+1) k / 2N)                              = scipy.fft.dct(x, 2) / 2
+ *   DCT3  X[k] = x[0] / 2 + sum_{n>=1} x[n] cos(pi n (2k+1) / 2N)            = scipy.fft.dct(x, 3) / 2
+ *   DCT4  X[k] = sum x[n] cos(pi (2n+1)(2k+1) / 4N)                          = scipy.fft.dct(x, 4) / 2
+ *   DST2  X[k] = sum x[n] sin(pi (2n+1)(k+1) / 2N)                           = scipy.fft.dst(x, 2) / 2
+ *   DST3  X[k] = (-1)^k x[N-1] / 2 + sum_{n<=N-2} x[n] sin(pi (n+1)(2k+1) / 2N) = scipy.fft.dst(x, 3) / 2
+ *   DST4  X[k] = sum x[n] sin(pi (2n+1)(2k+1) / 4N)                          = scipy.fft.dst(x, 4) / 2
+ * so DCT3(DCT2(x)) = DST3(DST2(x)) = DCT4(DCT4(x)) = DST4(DST4(x)) = (N/2) x.  len == 0 plans and is a silent no-op.
+ * len = 2^k with 4 <= len <= 32768 (f64: 16384) runs in one pass (one read and one write, no workspace; buffers aligned to two
+ * elements, B200FFT_ERR_INVALID_ARG otherwise).  Every other length runs a pre kernel, a complex plan and a post kernel over a
+ * workspace from the stream-ordered allocator: the len/2-point plan for even len, the len-point plan for odd len (DCT4 / DST4:
+ * 2 len points); a length whose complex plan cannot be built is B200FFT_ERR_UNSUPPORTED.  Any batch runs, in chunks where a launch would exceed its index range.  batch == 0 is a silent no-op.
+ * Plans are immutable and thread safe; the device entry point is asynchronous on the stream (CUDA-graph capturable). */
+typedef struct b200fft_dct_plan b200fft_dct_plan;
+enum { B200FFT_DCT2 = 0, B200FFT_DCT3 = 1, B200FFT_DCT4 = 2, B200FFT_DST2 = 3, B200FFT_DST3 = 4, B200FFT_DST4 = 5 };
+int b200fft_dct_plan_create(b200fft_dct_plan** out, uint64_t len, int kind, int precision, int device);
+int b200fft_dct_plan_destroy(b200fft_dct_plan* plan);
+/* e.g. "Dct2{n=4096,fused,M=2048}", "Dst4{n=1001,inner=Bluestein{...}}" (inner: the complex plan's description).  Returns length or <0. */
+int b200fft_dct_describe(const b200fft_dct_plan* plan, char* buf, uint64_t cap);
+/* d_in, d_out: batch * len reals on the plan's device; asynchronous on `cuda_stream`. */
+int b200fft_dct_device(const b200fft_dct_plan* plan, const void* d_in, void* d_out, uint64_t batch, void* cuda_stream);
+/* Same on host memory, synchronous (plain copies in and out, not pipelined). */
+int b200fft_dct_host(const b200fft_dct_plan* plan, const void* in, void* out, uint64_t batch);
+
 /* Message of the last failing call on this thread ("" if none). */
 const char* b200fft_last_error(void);
 /* Library build string: "b200fft <version> sm_90a" */

@@ -1,0 +1,97 @@
+//! `CudaDct<T>`: the DCT / DST plans of include/b200fft.h (`b200fft_dct_*`) in the shape of the `rustdct` crate's
+//! `Dct2` / `Dct3` / `Dct4` / `Dst2` / `Dst3` / `Dst4` traits (`process_dct2(&mut buffer)` ...), which sit on RustFFT's `Fft` the
+//! way `realfft` does.  Unnormalised like rustdct: DCT-III(DCT-II(x)) = (N/2) x.  NOT COMPILED IN THIS REPOSITORY (no rustc).
+
+use std::any::TypeId;
+use std::marker::PhantomData;
+use std::os::raw::{c_char, c_int, c_void};
+
+use crate::common::FftNum;
+
+#[repr(C)]
+pub struct B200FftDctPlan {
+    _private: [u8; 0],
+}
+
+/// `B200FFT_DCT2` ... `B200FFT_DST4`
+#[derive(Clone, Copy, Debug, PartialEq, Eq)]
+#[repr(i32)]
+pub enum DctKind {
+    Dct2 = 0,
+    Dct3 = 1,
+    Dct4 = 2,
+    Dst2 = 3,
+    Dst3 = 4,
+    Dst4 = 5,
+}
+
+#[link(name = "b200fft")]
+extern "C" {
+    fn b200fft_dct_plan_create(out: *mut *mut B200FftDctPlan, len: u64, kind: c_int, precision: c_int, device: c_int) -> c_int;
+    fn b200fft_dct_plan_destroy(plan: *mut B200FftDctPlan) -> c_int;
+    fn b200fft_dct_describe(plan: *const B200FftDctPlan, buf: *mut c_char, cap: u64) -> c_int;
+    fn b200fft_dct_host(plan: *const B200FftDctPlan, input: *const c_void, output: *mut c_void, batch: u64) -> c_int;
+}
+
+/// One planned DCT / DST of one length and kind on the GPU.  `Sync + Send`: the plan handle is immutable.
+pub struct CudaDct<T> {
+    plan: *mut B200FftDctPlan,
+    len: usize,
+    kind: DctKind,
+    _t: PhantomData<T>,
+}
+unsafe impl<T> Send for CudaDct<T> {}
+unsafe impl<T> Sync for CudaDct<T> {}
+
+impl<T: FftNum> CudaDct<T> {
+    pub fn new(len: usize, kind: DctKind) -> Result<Self, String> {
+        let precision = if TypeId::of::<T>() == TypeId::of::<f32>() { 0 } else if TypeId::of::<T>() == TypeId::of::<f64>() { 1 } else {
+            return Err("CudaDct supports f32 and f64 only".into());
+        };
+        let mut plan = std::ptr::null_mut();
+        let rc = unsafe { b200fft_dct_plan_create(&mut plan, len as u64, kind as c_int, precision, 0) };
+        if rc != 0 {
+            return Err(super::last_error_text());
+        }
+        Ok(Self { plan, len, kind, _t: PhantomData })
+    }
+    pub fn len(&self) -> usize {
+        self.len
+    }
+    pub fn kind(&self) -> DctKind {
+        self.kind
+    }
+    pub fn describe(&self) -> String {
+        let mut buf = vec![0u8; 512];
+        let n = unsafe { b200fft_dct_describe(self.plan, buf.as_mut_ptr().cast(), buf.len() as u64) };
+        if n < 0 {
+            return String::new();
+        }
+        buf.truncate(n as usize);
+        String::from_utf8_lossy(&buf).into_owned()
+    }
+    /// Every contiguous chunk of len() samples of `buffer`, in place (rustdct's `process_dct2(&mut buffer)` and friends; its
+    /// scratch variants need no scratch here).  Panics with the library's message, as rustdct panics on a bad length.
+    pub fn process(&self, buffer: &mut [T]) {
+        if self.len == 0 {
+            return;
+        }
+        assert!(buffer.len() % self.len == 0, "Dct: buffer holds {} samples, expected a multiple of {}", buffer.len(), self.len);
+        let rc = unsafe { b200fft_dct_host(self.plan, buffer.as_ptr().cast(), buffer.as_mut_ptr().cast(), (buffer.len() / self.len) as u64) };
+        if rc != 0 {
+            panic!("{}", super::last_error_text());
+        }
+    }
+    pub fn process_dct2(&self, buffer: &mut [T]) { debug_assert_eq!(self.kind, DctKind::Dct2); self.process(buffer) }
+    pub fn process_dct3(&self, buffer: &mut [T]) { debug_assert_eq!(self.kind, DctKind::Dct3); self.process(buffer) }
+    pub fn process_dct4(&self, buffer: &mut [T]) { debug_assert_eq!(self.kind, DctKind::Dct4); self.process(buffer) }
+    pub fn process_dst2(&self, buffer: &mut [T]) { debug_assert_eq!(self.kind, DctKind::Dst2); self.process(buffer) }
+    pub fn process_dst3(&self, buffer: &mut [T]) { debug_assert_eq!(self.kind, DctKind::Dst3); self.process(buffer) }
+    pub fn process_dst4(&self, buffer: &mut [T]) { debug_assert_eq!(self.kind, DctKind::Dst4); self.process(buffer) }
+}
+
+impl<T> Drop for CudaDct<T> {
+    fn drop(&mut self) {
+        unsafe { b200fft_dct_plan_destroy(self.plan) };
+    }
+}

@@ -13,6 +13,7 @@ use num_complex::Complex;
 use crate::common::FftNum;
 use crate::{Direction, Fft, FftDirection, Length};
 
+pub mod cuda_dct;
 pub mod cuda_planner;
 
 #[repr(C)]

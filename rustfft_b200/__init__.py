@@ -27,7 +27,7 @@ from typing import Dict, Optional, Tuple
 import numpy as np
 
 __all__ = ["FftDirection", "FftPlanner", "Fft", "Library", "FftError", "Recipe", "RealFftPlanner", "RealFft", "RealFft2d", "Fft2d", "FftConvolution",
-           "FftConvolution2d",
+           "FftConvolution2d", "DctKind", "DctPlanner", "Dct",
            "default_library", "shard_range"]
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -135,6 +135,7 @@ class Library:
         "b200fft_real2d_inverse_device", "b200fft_real2d_forward_host", "b200fft_real2d_inverse_host",
         "b200fft_conv2d_plan_create", "b200fft_conv2d_plan_destroy", "b200fft_conv2d_output_shape", "b200fft_conv2d_describe",
         "b200fft_conv2d_device", "b200fft_conv2d_host",
+        "b200fft_dct_plan_create", "b200fft_dct_plan_destroy", "b200fft_dct_describe", "b200fft_dct_device", "b200fft_dct_host",
     ]
 
     def __init__(self, path: str = DEFAULT_LIB_PATH):
@@ -198,6 +199,11 @@ class Library:
         c.b200fft_conv2d_describe.argtypes = [vp, ctypes.c_char_p, u64]
         c.b200fft_conv2d_device.argtypes = [vp, vp, vp, u64, vp]
         c.b200fft_conv2d_host.argtypes = [vp, vp, vp, u64]
+        c.b200fft_dct_plan_create.argtypes = [ctypes.POINTER(vp), u64, i32, i32, i32]
+        c.b200fft_dct_plan_destroy.argtypes = [vp]
+        c.b200fft_dct_describe.argtypes = [vp, ctypes.c_char_p, u64]
+        c.b200fft_dct_device.argtypes = [vp, vp, vp, u64, vp]
+        c.b200fft_dct_host.argtypes = [vp, vp, vp, u64]
 
     def device_count(self) -> int:
         n = ctypes.c_int(0)
@@ -815,6 +821,147 @@ class FftConvolution2d:
         self._lib.check(self._lib.c.b200fft_conv2d_device(self._h, x.data_ptr(), out.data_ptr(), batch,
                                                           torch.cuda.current_stream(x.device).cuda_stream))
         return out
+
+
+class DctKind(enum.IntEnum):
+    """The rustdct traits a plan implements (B200FFT_DCT2 ... B200FFT_DST4)."""
+    Dct2 = 0
+    Dct3 = 1
+    Dct4 = 2
+    Dst2 = 3
+    Dst3 = 4
+    Dst4 = 5
+
+
+class Dct:
+    """One planned DCT or DST of one length (the shape of rustdct's Dct2 / Dct3 / Dct4 / Dst2 / Dst3 / Dst4 over RustFFT's Fft):
+    every contiguous row of len() reals is transformed, unnormalised, as scipy.fft.dct / dst(x, type) / 2:
+
+        Dct2  X[k] = sum x[n] cos(pi (2n+1) k / 2N)             Dst2  X[k] = sum x[n] sin(pi (2n+1)(k+1) / 2N)
+        Dct3  X[k] = x[0]/2 + sum_{n>=1} x[n] cos(pi n (2k+1) / 2N)
+        Dst3  X[k] = (-1)^k x[N-1]/2 + sum_{n<=N-2} x[n] sin(pi (n+1)(2k+1) / 2N)
+        Dct4  X[k] = sum x[n] cos(pi (2n+1)(2k+1) / 4N)         Dst4  X[k] = sum x[n] sin(pi (2n+1)(2k+1) / 4N)
+
+    so Dct3(Dct2(x)) = Dst3(Dst2(x)) = Dct4(Dct4(x)) = Dst4(Dst4(x)) = (N/2) x.  Powers of two from 4 to 32768 (f64: 16384) run in
+    one pass, which moves element pairs: its device buffers must start at an even element (a torch view such as x[1:] of an
+    allocation does not; process_device raises TypeError for it).  Other lengths run around a complex plan and take any offset.  process(buffer) transforms a numpy array in place through the synchronous
+    host entry point; process_device(x, out=None) takes torch CUDA tensors, in place when out is None, asynchronous on torch's
+    current stream.  Immutable and safe to call from many threads."""
+
+    def __init__(self, lib: Library, length: int, kind: DctKind, precision: int, device: int):
+        self._lib, self._len, self._kind, self._precision, self.device = lib, int(length), DctKind(kind), precision, device
+        self._h = ctypes.c_void_p()
+        lib.check(lib.c.b200fft_dct_plan_create(ctypes.byref(self._h), self._len, int(kind), precision, device))
+        self._fused = ",fused," in self.describe()
+
+    def __del__(self):
+        h, self._h = getattr(self, "_h", None), None
+        if h:
+            try:
+                self._lib.c.b200fft_dct_plan_destroy(h)
+            except Exception:
+                pass
+
+    def len(self) -> int:
+        return self._len
+
+    def __len__(self) -> int:
+        return self._len
+
+    def kind(self) -> DctKind:
+        return self._kind
+
+    @property
+    def dtype(self):
+        return np.float32 if self._precision == F32 else np.float64
+
+    def describe(self) -> str:
+        buf = ctypes.create_string_buffer(512)
+        rc = self._lib.c.b200fft_dct_describe(self._h, buf, len(buf))
+        if rc < 0:
+            self._lib.check(rc)
+        return buf.value.decode()
+
+    def _batch(self, n: int) -> int:
+        if self._len == 0:
+            return 0
+        if n % self._len:
+            raise FftError(-5, f"Dct: buffer holds {n} samples, expected a multiple of {self._len}")
+        return n // self._len
+
+    def process(self, buffer: np.ndarray) -> np.ndarray:
+        """Transform every row of `buffer` (batch * len() reals, contiguous, writable) in place; returns it."""
+        want = np.dtype(self.dtype)
+        if not isinstance(buffer, np.ndarray) or buffer.dtype != want or not buffer.flags.c_contiguous or not buffer.flags.writeable:
+            raise TypeError(f"Dct.process wants a contiguous writable {want.name} array")
+        batch = self._batch(buffer.size)
+        self._lib.check(self._lib.c.b200fft_dct_host(self._h, buffer.ctypes.data, buffer.ctypes.data, batch))
+        return buffer
+
+    def process_device(self, x, out=None):
+        """x: torch CUDA tensor of batch * len() reals (any shape, contiguous); in place when `out` is None.  Returns the result."""
+        import torch
+
+        want = torch.float32 if self._precision == F32 else torch.float64
+        dst = x if out is None else out
+        if not isinstance(dst, torch.Tensor) or x.dtype != want or dst.dtype != want or not x.is_cuda or not dst.is_cuda \
+                or not x.is_contiguous() or not dst.is_contiguous():
+            raise TypeError(f"Dct.process_device wants contiguous CUDA tensors of {want}")
+        if x.device.index != self.device or dst.device.index != self.device:
+            raise FftError(-1, f"tensors are on cuda:{x.device.index} / cuda:{dst.device.index}, plan is on cuda:{self.device}")
+        if dst.numel() != x.numel():
+            raise FftError(-6, f"Dct: input holds {x.numel()} samples, output {dst.numel()}: expected equal sizes")
+        if self._fused and (x.data_ptr() | dst.data_ptr()) % (2 * x.element_size()):
+            raise TypeError("Dct.process_device: a one-pass plan needs tensors that start at an even element (it moves element pairs)")
+        batch = self._batch(x.numel())
+        self._lib.check(self._lib.c.b200fft_dct_device(self._h, x.data_ptr(), dst.data_ptr(), batch,
+                                                       torch.cuda.current_stream(x.device).cuda_stream))
+        return dst
+
+
+class DctPlanner:
+    """Plans Dct instances, cached per (kind, length) like rustdct's DctPlanner over rustfft's FftPlanner."""
+
+    def __init__(self, dtype=np.float32, device: int = 0, lib: Optional[Library] = None):
+        dt = np.dtype(dtype)
+        if dt == np.dtype(np.float32):
+            self._precision = F32
+        elif dt == np.dtype(np.float64):
+            self._precision = F64
+        else:
+            raise TypeError("DctPlanner accelerates f32 and f64 only")
+        self._lib = lib if lib is not None else default_library()
+        if self._lib.device_count() <= 0:
+            raise FftError(-2, "no sm_90 CUDA device is visible (there is no CPU fallback)")
+        self.device = device
+        self._cache: Dict[Tuple[int, int], Dct] = {}
+        self._lock = threading.Lock()
+
+    def plan(self, kind: DctKind, len: int) -> Dct:
+        key = (int(kind), int(len))
+        with self._lock:
+            d = self._cache.get(key)
+            if d is None:
+                d = self._cache[key] = Dct(self._lib, key[1], DctKind(kind), self._precision, self.device)
+            return d
+
+    def plan_dct2(self, len: int) -> Dct:
+        return self.plan(DctKind.Dct2, len)
+
+    def plan_dct3(self, len: int) -> Dct:
+        return self.plan(DctKind.Dct3, len)
+
+    def plan_dct4(self, len: int) -> Dct:
+        return self.plan(DctKind.Dct4, len)
+
+    def plan_dst2(self, len: int) -> Dct:
+        return self.plan(DctKind.Dst2, len)
+
+    def plan_dst3(self, len: int) -> Dct:
+        return self.plan(DctKind.Dst3, len)
+
+    def plan_dst4(self, len: int) -> Dct:
+        return self.plan(DctKind.Dst4, len)
 
 
 def shard_range(batch: int, rank: int, world: int) -> Tuple[int, int]:
