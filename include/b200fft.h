@@ -269,6 +269,29 @@ int b200fft_dct_device(const b200fft_dct_plan* plan, const void* d_in, void* d_o
 /* Same on host memory, synchronous (plain copies in and out, not pipelined). */
 int b200fft_dct_host(const b200fft_dct_plan* plan, const void* in, void* out, uint64_t batch);
 
+/* Batched 2-D and 3-D DCTs / DSTs: the same kind (B200FFT_DCT2 .. B200FFT_DST4) along each of the last `rank` (2 or 3) axes of
+ * contiguous row-major arrays of shape[0] x .. x shape[rank-1] reals; a buffer holds `batch` such arrays.  Unnormalised: the result
+ * is scipy.fft.dctn / dstn(x, type, axes = the last rank axes) / 2^rank, so DCT3n(DCT2n(x)) = DST3n(DST2n(x)) = DCT4n(DCT4n(x)) =
+ * DST4n(DST4n(x)) = prod(shape[i] / 2) x.  Every axis length the 1-D plan of that kind accepts is supported; an axis whose 1-D plan
+ * cannot be built is that plan's error, prefixed with the axis.  Arrays of zero elements and batch == 0 are silent no-ops.
+ * The last axis runs the 1-D plan over every row (in -> out); every other axis then runs in place on out, one pass per axis: a
+ * fused column pass for power-of-two lengths 4 .. 4096 (f64: 2048), one read and one write with no workspace; any other length
+ * transposes slabs into a workspace from the stream-ordered allocator, runs the 1-D plan there and transposes back.
+ * d_in == d_out (in place) is allowed; any other overlap is B200FFT_ERR_INVALID_ARG.  When the last axis runs a fused 1-D plan the
+ * buffers must be aligned to two elements (B200FFT_ERR_INVALID_ARG otherwise).  Plans are immutable and thread safe; the device
+ * entry point is asynchronous on the stream (CUDA-graph capturable). */
+typedef struct b200fft_dctn_plan b200fft_dctn_plan;
+int b200fft_dctn_plan_create(b200fft_dctn_plan** out, const uint64_t* shape, int rank, int kind, int precision, int device);
+int b200fft_dctn_plan_destroy(b200fft_dctn_plan* plan);
+/* e.g. "Dct2{512x512,rows=Dct2{n=512,fused,M=256},cols=fused{M=256,F=16}}",
+ * "Dst3{1080x1920,rows=Dst3{n=1920,inner=...},cols=transposed{Dst3{n=1080,inner=...}}}": the last axis first (3-D: rows, cols,
+ * then depth).  Returns length or <0. */
+int b200fft_dctn_describe(const b200fft_dctn_plan* plan, char* buf, uint64_t cap);
+/* d_in, d_out: batch * prod(shape) reals on the plan's device; asynchronous on `cuda_stream`. */
+int b200fft_dctn_device(const b200fft_dctn_plan* plan, const void* d_in, void* d_out, uint64_t batch, void* cuda_stream);
+/* Same on host memory, synchronous (plain copies in and out, not pipelined). */
+int b200fft_dctn_host(const b200fft_dctn_plan* plan, const void* in, void* out, uint64_t batch);
+
 /* Message of the last failing call on this thread ("" if none). */
 const char* b200fft_last_error(void);
 /* Library build string: "b200fft <version> sm_90a" */

@@ -95,3 +95,76 @@ impl<T> Drop for CudaDct<T> {
         unsafe { b200fft_dct_plan_destroy(self.plan) };
     }
 }
+
+#[repr(C)]
+pub struct B200FftDctnPlan {
+    _private: [u8; 0],
+}
+
+#[link(name = "b200fft")]
+extern "C" {
+    fn b200fft_dctn_plan_create(out: *mut *mut B200FftDctnPlan, shape: *const u64, rank: c_int, kind: c_int, precision: c_int, device: c_int) -> c_int;
+    fn b200fft_dctn_plan_destroy(plan: *mut B200FftDctnPlan) -> c_int;
+    fn b200fft_dctn_describe(plan: *const B200FftDctnPlan, buf: *mut c_char, cap: u64) -> c_int;
+    fn b200fft_dctn_host(plan: *const B200FftDctnPlan, input: *const c_void, output: *mut c_void, batch: u64) -> c_int;
+}
+
+/// One planned 2-D or 3-D DCT / DST (`b200fft_dctn_*`): the same kind along each of the last `shape.len()` axes of contiguous
+/// row-major arrays, unnormalised (= scipy.fft.dctn / dstn / 2^rank).  `Sync + Send`: the plan handle is immutable.
+pub struct CudaDctNd<T> {
+    plan: *mut B200FftDctnPlan,
+    shape: Vec<usize>,
+    kind: DctKind,
+    _t: PhantomData<T>,
+}
+unsafe impl<T> Send for CudaDctNd<T> {}
+unsafe impl<T> Sync for CudaDctNd<T> {}
+
+impl<T: FftNum> CudaDctNd<T> {
+    /// `shape`: 2 or 3 axis lengths, each one the 1-D plan of `kind` accepts.
+    pub fn new(shape: &[usize], kind: DctKind) -> Result<Self, String> {
+        let precision = if TypeId::of::<T>() == TypeId::of::<f32>() { 0 } else if TypeId::of::<T>() == TypeId::of::<f64>() { 1 } else {
+            return Err("CudaDctNd supports f32 and f64 only".into());
+        };
+        let dims: Vec<u64> = shape.iter().map(|&n| n as u64).collect();
+        let mut plan = std::ptr::null_mut();
+        let rc = unsafe { b200fft_dctn_plan_create(&mut plan, dims.as_ptr(), dims.len() as c_int, kind as c_int, precision, 0) };
+        if rc != 0 {
+            return Err(super::last_error_text());
+        }
+        Ok(Self { plan, shape: shape.to_vec(), kind, _t: PhantomData })
+    }
+    pub fn shape(&self) -> &[usize] {
+        &self.shape
+    }
+    pub fn kind(&self) -> DctKind {
+        self.kind
+    }
+    pub fn describe(&self) -> String {
+        let mut buf = vec![0u8; 1024];
+        let n = unsafe { b200fft_dctn_describe(self.plan, buf.as_mut_ptr().cast(), buf.len() as u64) };
+        if n < 0 {
+            return String::new();
+        }
+        buf.truncate(n as usize);
+        String::from_utf8_lossy(&buf).into_owned()
+    }
+    /// Every contiguous array of `shape` in `buffer`, in place.  Panics with the library's message on a bad length.
+    pub fn process(&self, buffer: &mut [T]) {
+        let size: usize = self.shape.iter().product();
+        if size == 0 {
+            return;
+        }
+        assert!(buffer.len() % size == 0, "DctNd: buffer holds {} samples, expected a multiple of {}", buffer.len(), size);
+        let rc = unsafe { b200fft_dctn_host(self.plan, buffer.as_ptr().cast(), buffer.as_mut_ptr().cast(), (buffer.len() / size) as u64) };
+        if rc != 0 {
+            panic!("{}", super::last_error_text());
+        }
+    }
+}
+
+impl<T> Drop for CudaDctNd<T> {
+    fn drop(&mut self) {
+        unsafe { b200fft_dctn_plan_destroy(self.plan) };
+    }
+}

@@ -21,13 +21,14 @@ from __future__ import annotations
 import ctypes
 import enum
 import os
+import re
 import threading
 from typing import Dict, Optional, Tuple
 
 import numpy as np
 
 __all__ = ["FftDirection", "FftPlanner", "Fft", "Library", "FftError", "Recipe", "RealFftPlanner", "RealFft", "RealFft2d", "Fft2d", "FftConvolution",
-           "FftConvolution2d", "DctKind", "DctPlanner", "Dct",
+           "FftConvolution2d", "DctKind", "DctPlanner", "Dct", "DctNd",
            "default_library", "shard_range"]
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -136,6 +137,7 @@ class Library:
         "b200fft_conv2d_plan_create", "b200fft_conv2d_plan_destroy", "b200fft_conv2d_output_shape", "b200fft_conv2d_describe",
         "b200fft_conv2d_device", "b200fft_conv2d_host",
         "b200fft_dct_plan_create", "b200fft_dct_plan_destroy", "b200fft_dct_describe", "b200fft_dct_device", "b200fft_dct_host",
+        "b200fft_dctn_plan_create", "b200fft_dctn_plan_destroy", "b200fft_dctn_describe", "b200fft_dctn_device", "b200fft_dctn_host",
     ]
 
     def __init__(self, path: str = DEFAULT_LIB_PATH):
@@ -204,6 +206,11 @@ class Library:
         c.b200fft_dct_describe.argtypes = [vp, ctypes.c_char_p, u64]
         c.b200fft_dct_device.argtypes = [vp, vp, vp, u64, vp]
         c.b200fft_dct_host.argtypes = [vp, vp, vp, u64]
+        c.b200fft_dctn_plan_create.argtypes = [ctypes.POINTER(vp), ctypes.POINTER(u64), i32, i32, i32, i32]
+        c.b200fft_dctn_plan_destroy.argtypes = [vp]
+        c.b200fft_dctn_describe.argtypes = [vp, ctypes.c_char_p, u64]
+        c.b200fft_dctn_device.argtypes = [vp, vp, vp, u64, vp]
+        c.b200fft_dctn_host.argtypes = [vp, vp, vp, u64]
 
     def device_count(self) -> int:
         n = ctypes.c_int(0)
@@ -919,8 +926,90 @@ class Dct:
         return dst
 
 
+class DctNd:
+    """One planned 2-D or 3-D DCT or DST: the same kind along each of the last len(shape()) axes of contiguous arrays of shape(),
+    unnormalised, as scipy.fft.dctn / dstn(x, type, axes=the last r axes) / 2^r, so that Dct3n(Dct2n(x)) = Dst3n(Dst2n(x)) =
+    Dct4n(Dct4n(x)) = Dst4n(Dst4n(x)) = prod(N_i / 2) x.  The last axis runs the 1-D plan of its length; every other axis runs one
+    fused column pass for powers of two from 4 to 4096 (f64: 2048), or a transposition around the 1-D plan of its length.  When the
+    last axis is a one-pass 1-D plan, device buffers must start at an even element (process_device raises TypeError otherwise).
+    process(buffer) transforms a numpy array of whole images in place through the synchronous host entry point;
+    process_device(x, out=None) takes torch CUDA tensors, in place when out is None, asynchronous on torch's current stream.
+    Immutable and safe to call from many threads."""
+
+    def __init__(self, lib: Library, shape, kind: DctKind, precision: int, device: int):
+        self._lib, self._shape, self._kind, self._precision, self.device = lib, tuple(int(n) for n in shape), DctKind(kind), precision, device
+        self._size = int(np.prod(self._shape, dtype=np.int64)) if self._shape else 0
+        self._h = ctypes.c_void_p()
+        dims = (ctypes.c_uint64 * max(1, len(self._shape)))(*self._shape)
+        lib.check(lib.c.b200fft_dctn_plan_create(ctypes.byref(self._h), dims, len(self._shape), int(kind), precision, device))
+        rows = self.describe().split(",rows=", 1)
+        self._fused = len(rows) == 2 and re.match(r"\w+\{n=\d+,fused,", rows[1]) is not None
+
+    def __del__(self):
+        h, self._h = getattr(self, "_h", None), None
+        if h:
+            try:
+                self._lib.c.b200fft_dctn_plan_destroy(h)
+            except Exception:
+                pass
+
+    def shape(self) -> Tuple[int, ...]:
+        return self._shape
+
+    def kind(self) -> DctKind:
+        return self._kind
+
+    @property
+    def dtype(self):
+        return np.float32 if self._precision == F32 else np.float64
+
+    def describe(self) -> str:
+        buf = ctypes.create_string_buffer(1024)
+        rc = self._lib.c.b200fft_dctn_describe(self._h, buf, len(buf))
+        if rc < 0:
+            self._lib.check(rc)
+        return buf.value.decode()
+
+    def _batch(self, n: int) -> int:
+        if self._size == 0:
+            return 0
+        if n % self._size:
+            raise FftError(-5, f"DctNd: buffer holds {n} samples, expected a multiple of {self._size}")
+        return n // self._size
+
+    def process(self, buffer: np.ndarray) -> np.ndarray:
+        """Transform every array of `buffer` (batch * prod(shape()) reals, contiguous, writable) in place; returns it."""
+        want = np.dtype(self.dtype)
+        if not isinstance(buffer, np.ndarray) or buffer.dtype != want or not buffer.flags.c_contiguous or not buffer.flags.writeable:
+            raise TypeError(f"DctNd.process wants a contiguous writable {want.name} array")
+        batch = self._batch(buffer.size)
+        self._lib.check(self._lib.c.b200fft_dctn_host(self._h, buffer.ctypes.data, buffer.ctypes.data, batch))
+        return buffer
+
+    def process_device(self, x, out=None):
+        """x: torch CUDA tensor of batch * prod(shape()) reals (any shape, contiguous); in place when `out` is None.  Returns the result."""
+        import torch
+
+        want = torch.float32 if self._precision == F32 else torch.float64
+        dst = x if out is None else out
+        if not isinstance(dst, torch.Tensor) or x.dtype != want or dst.dtype != want or not x.is_cuda or not dst.is_cuda \
+                or not x.is_contiguous() or not dst.is_contiguous():
+            raise TypeError(f"DctNd.process_device wants contiguous CUDA tensors of {want}")
+        if x.device.index != self.device or dst.device.index != self.device:
+            raise FftError(-1, f"tensors are on cuda:{x.device.index} / cuda:{dst.device.index}, plan is on cuda:{self.device}")
+        if dst.numel() != x.numel():
+            raise FftError(-6, f"DctNd: input holds {x.numel()} samples, output {dst.numel()}: expected equal sizes")
+        if self._fused and (x.data_ptr() | dst.data_ptr()) % (2 * x.element_size()):
+            raise TypeError("DctNd.process_device: a one-pass row plan needs tensors that start at an even element (it moves element pairs)")
+        batch = self._batch(x.numel())
+        self._lib.check(self._lib.c.b200fft_dctn_device(self._h, x.data_ptr(), dst.data_ptr(), batch,
+                                                        torch.cuda.current_stream(x.device).cuda_stream))
+        return dst
+
+
 class DctPlanner:
-    """Plans Dct instances, cached per (kind, length) like rustdct's DctPlanner over rustfft's FftPlanner."""
+    """Plans Dct instances, cached per (kind, length) like rustdct's DctPlanner over rustfft's FftPlanner, and DctNd instances
+    (plan_nd), cached per (kind, shape)."""
 
     def __init__(self, dtype=np.float32, device: int = 0, lib: Optional[Library] = None):
         dt = np.dtype(dtype)
@@ -935,6 +1024,7 @@ class DctPlanner:
             raise FftError(-2, "no sm_90 CUDA device is visible (there is no CPU fallback)")
         self.device = device
         self._cache: Dict[Tuple[int, int], Dct] = {}
+        self._cache_nd: Dict[Tuple[int, Tuple[int, ...]], DctNd] = {}
         self._lock = threading.Lock()
 
     def plan(self, kind: DctKind, len: int) -> Dct:
@@ -943,6 +1033,15 @@ class DctPlanner:
             d = self._cache.get(key)
             if d is None:
                 d = self._cache[key] = Dct(self._lib, key[1], DctKind(kind), self._precision, self.device)
+            return d
+
+    def plan_nd(self, kind: DctKind, shape) -> DctNd:
+        """The same kind along each of the last len(shape) (2 or 3) axes of contiguous arrays of `shape`."""
+        key = (int(kind), tuple(int(n) for n in shape))
+        with self._lock:
+            d = self._cache_nd.get(key)
+            if d is None:
+                d = self._cache_nd[key] = DctNd(self._lib, key[1], DctKind(kind), self._precision, self.device)
             return d
 
     def plan_dct2(self, len: int) -> Dct:

@@ -299,4 +299,165 @@ struct DctGenKernel {
     }
 };
 
+// DctAxisKernel<G, KIND>: DctKernel<G, KIND> down a strided axis, for the 2-D / 3-D transforms.  The data is viewed as
+// [outer][N][inner] (N = 2M, M = G::L); column g = o inner + c (o < outer, c < inner) holds element n at o N inner + n inner + c.  A CTA
+// takes the F adjacent columns g0 .. g0 + F - 1 (a tile may span slabs, and in a launch's last CTA it may end early):
+//   phase 0      the [N][F] tile from global memory, a warp reading runs of F adjacent columns per row (coalesced), into registers,
+//                then into a staging layout of the same buffer: element (n, f) at real n F + ((f + rot(n)) mod F)
+//   phase 1      the staging layout into registers: thread t's slot k is real t + NT k of the layout below or, where a column
+//                spans at least a 128-byte run of threads (BY_COLUMN), row t mod RS + RS k of column t / RS (RS = NT / F)
+//   phase 2      registers into DctKernel's layout: column f at reals [f N, (f + 1) N)
+//   then DctKernel's phases 1 .. NPHASE - 2 (build, M-point engine, combine) unchanged, on an embedded DctKernel::Params,
+//   and the reverse: DctKernel's layout -> registers -> staging -> registers -> global memory.
+// rot(n) = n max(1, B/N) / max(1, B/F), B = reals per 128 bytes: a warp's accesses of the staging in either order fall on distinct
+// banks, and DctKernel's layout is accessed at consecutive reals (tests/test_dctn.py enumerates every warp access of both).  In the
+// column order every address of a thread is one base plus compile-time offsets; the order of DctKernel's layout made f32 M >= 256
+// spill (each slot's staging address computed separately).  Every CTA reads its whole tile before it stores, so in place is safe;
+// no workspace.
+template <class G, int KIND>
+struct DctAxisKernel {
+    using T = typename G::T;
+    using DK = DctKernel<G, KIND>;
+    static constexpr int M = G::L, N = 2 * G::L, F = G::F, NT = G::NT;
+    static constexpr int K = N * F / NT;  // reals per thread in the load and the store (2 E: DctKernel's registers)
+    static constexpr int RS = NT / F;     // rows of the tile one load / store slot covers
+    static constexpr int B = 128 / (int)sizeof(T);
+    static constexpr int ROT_MUL = N < B ? B / N : 1, ROT_DIV = F < B ? B / F : 1;
+    // column order in phases 1 / 2 and their reverse: a warp's run of B threads stays in one column, and row n + RS k of a column is
+    // staged RS F k reals after row n (RS / ROT_DIV, the rotation's step, is a multiple of F)
+    static constexpr bool BY_COLUMN = RS >= B && (RS / ROT_DIV) % F == 0;
+    // the same step for the rows of the load and the store: row n0 + RS k of a column staged RS F k reals after row n0
+    static constexpr bool ROW_STEP = (RS * ROT_MUL) % ROT_DIV == 0 && (RS * ROT_MUL / ROT_DIV) % F == 0;
+    static constexpr int MIN_BLOCKS = DK::MIN_BLOCKS;
+    static constexpr int P_DK = 2;                       // DctKernel's phase P (1 .. DK::NPHASE - 2) runs as phase P + P_DK
+    static constexpr int P_OUT = DK::NPHASE - 1 + P_DK;  // first phase of the store
+    static constexpr int NPHASE = P_OUT + 3;
+    static constexpr size_t SMEM_BYTES = DK::SMEM_BYTES;
+    static_assert(K == 2 * G::E && NT % F == 0 && (F & (F - 1)) == 0, "the tile must split evenly over the threads");
+    static_assert((size_t)N * F * sizeof(T) <= SMEM_BYTES, "the tile must fit DctKernel's buffer");
+    struct Params {
+        typename DK::Params dk;  // DctKernel's tables (its in / out / rows are not used)
+        const T* in;
+        T* out;
+        uint64_t cols;       // columns in this launch (cols + F < 2^31)
+        uint64_t slab;       // elements between slabs: N inner
+        uint64_t row;        // elements between the rows of a column: inner
+        FastDiv div_inner;   // g -> (o, c); a launch inside one slab divides by 2^30 (o = 0)
+    };
+    using Regs = typename DK::Regs;
+
+    static B2_HD int stage(int n, int f) { return n * F + ((f + n * ROT_MUL / ROT_DIV) & (F - 1)); }
+    static B2_HD T& reg(Regs& r, int k) { return (k & 1) ? r.v[k >> 1].y : r.v[k >> 1].x; }
+    // staging real of the load's / store's slot k (row tid / F + RS k of column tid mod F)
+    static B2_HD int row_slot(int tid, int k) {
+        if constexpr (ROW_STEP) return stage(tid / F, tid & (F - 1)) + RS * F * k;
+        else return stage(tid / F + RS * k, tid & (F - 1));
+    }
+    // slot k of thread tid in phases 1 / 2 and their reverse: its real in DctKernel's layout and in the staging layout
+    static B2_HD void slot(int tid, int k, int& fin, int& stg) {
+        if constexpr (BY_COLUMN) {
+            const int f = tid / RS, j = tid % RS;
+            fin = f * N + j + RS * k;
+            stg = stage(j, f) + RS * F * k;
+        } else {
+            const int i = tid + NT * k;
+            fin = i;
+            stg = stage(i % N, i / N);
+        }
+    }
+    // offset of row tid / F of this thread's column g0 + tid mod F
+    static B2_HD uint64_t origin(const Params& p, uint32_t bid, int tid) {
+        const uint32_t g = bid * F + (tid & (F - 1)), o = p.div_inner.div(g);
+        return (uint64_t)o * p.slab + (g - o * p.div_inner.d) + (uint64_t)(tid / F) * p.row;
+    }
+    static B2_HD bool whole(const Params& p, uint32_t bid) { return (uint64_t)bid * F + F <= p.cols; }
+    static B2_HD bool live(const Params& p, uint32_t bid, int tid) { return (uint64_t)bid * F + (tid & (F - 1)) < p.cols; }
+
+    template <int P>
+    static B2_HD void phase(const Params& p, uint32_t bid, int tid, Regs& r, cx<T>* smem) {
+        T* s = reinterpret_cast<T*>(smem);
+        if constexpr (P == 0) {
+            // (only a launch's last CTA tests its columns; one test per thread: a thread keeps one column)
+            if (whole(p, bid) || live(p, bid, tid)) {
+                const T* src = p.in + origin(p, bid, tid);
+                const uint64_t step = (uint64_t)RS * p.row;
+                B2_UNROLL
+                for (int k = 0; k < K; ++k) reg(r, k) = src[k * step];
+            } else {
+                B2_UNROLL
+                for (int k = 0; k < K; ++k) reg(r, k) = (T)0;
+            }
+            B2_UNROLL
+            for (int k = 0; k < K; ++k) s[row_slot(tid, k)] = reg(r, k);
+        }
+        if constexpr (P == 1 || P == 2 || P == P_OUT || P == P_OUT + 1) {
+            B2_UNROLL
+            for (int k = 0; k < K; ++k) {
+                int fin, stg;
+                slot(tid, k, fin, stg);
+                if constexpr (P == 1) reg(r, k) = s[stg];
+                if constexpr (P == 2) s[fin] = reg(r, k);
+                if constexpr (P == P_OUT) reg(r, k) = s[fin];
+                if constexpr (P == P_OUT + 1) s[stg] = reg(r, k);
+            }
+        }
+        if constexpr (P > P_DK && P < P_OUT) DK::template phase<P - P_DK>(p.dk, bid, tid, r, smem);
+        if constexpr (P == P_OUT + 2) {
+            B2_UNROLL
+            for (int k = 0; k < K; ++k) reg(r, k) = s[row_slot(tid, k)];
+            if (whole(p, bid) || live(p, bid, tid)) {
+                T* dst = p.out + origin(p, bid, tid);
+                const uint64_t step = (uint64_t)RS * p.row;
+                B2_UNROLL
+                for (int k = 0; k < K; ++k) dst[k * step] = reg(r, k);
+            }
+        }
+    }
+};
+
+// DctTransposeKernel<T>: out[s os + c ol + r] = in[s is + r il + c] for r < R, c < C, s < slabs: the transposition of each [R][C] slab
+// around the 1-D plan on the N-D transforms' other route.  32 x 32 tiles through shared memory padded to a pitch of 33, 256 threads;
+// reads along c and writes along r are coalesced, and both shared-memory sides are free of bank conflicts (tests/test_dctn.py).
+template <typename TT>
+struct DctTransposeKernel {
+    using T = TT;
+    static constexpr int TILE = 32, PITCH = TILE + 1;
+    static constexpr int NT = 256;
+    static constexpr int MIN_BLOCKS = 4;
+    static constexpr int NPHASE = 2;
+    static constexpr size_t SMEM_BYTES = sizeof(T) * TILE * PITCH;
+    struct Params {
+        const T* in;
+        T* out;
+        uint32_t R, C;     // rows and columns of a slab
+        uint32_t tr, tc;   // tiles along R and C
+        uint64_t is, il;   // input: elements between slabs, between rows
+        uint64_t os, ol;   // output: elements between slabs, between columns
+    };
+    struct Regs {};
+    template <int P>
+    static B2_HD void phase(const Params& p, uint32_t bid, int tid, Regs&, cx<T>* smem) {
+        T* tile = reinterpret_cast<T*>(smem);
+        const uint32_t bc = bid % p.tc, t = bid / p.tc, br = t % p.tr, sl = t / p.tr;
+        const int x = tid % TILE, y = tid / TILE;
+        if constexpr (P == 0) {
+            const uint32_t c = bc * TILE + x;
+            const T* src = p.in + sl * p.is + c;
+            B2_UNROLL
+            for (int i = 0; i < TILE; i += NT / TILE) {
+                const uint32_t r = br * TILE + y + i;
+                if (r < p.R && c < p.C) tile[(y + i) * PITCH + x] = src[r * p.il];
+            }
+        } else {
+            const uint32_t r = br * TILE + x;
+            T* dst = p.out + sl * p.os + r;
+            B2_UNROLL
+            for (int i = 0; i < TILE; i += NT / TILE) {
+                const uint32_t c = bc * TILE + y + i;
+                if (r < p.R && c < p.C) dst[c * p.ol] = tile[x * PITCH + y + i];
+            }
+        }
+    }
+};
+
 }  // namespace b2
