@@ -292,6 +292,46 @@ int b200fft_dctn_device(const b200fft_dctn_plan* plan, const void* d_in, void* d
 /* Same on host memory, synchronous (plain copies in and out, not pipelined). */
 int b200fft_dctn_host(const b200fft_dctn_plan* plan, const void* in, void* out, uint64_t batch);
 
+/* Batched short-time Fourier transforms of real rows.  A plan fixes a real `window` of n_fft taps (host memory, in the plan's
+ * precision; n_fft even and >= 2), the hop (1 <= hop <= n_fft), signal_len and `center`.  A signal buffer holds batch contiguous
+ * rows of signal_len reals; a spectrum buffer holds batch * frames * (n_fft/2 + 1) complex values, frame-major: row r, frame f,
+ * bin k at (r frames + f) (n_fft/2 + 1) + k (torch.stft's [bins][frames] layout is the transpose of the last two axes).
+ *   forward  S[f][k] = sum_u w[u] xp[f hop + u] exp(-2 pi i k u / n_fft),  u < n_fft, k <= n_fft/2   (unnormalised)
+ *            xp = x reflect-padded by n_fft/2 on each side when center (torch's pad_mode "reflect"; needs signal_len > n_fft/2),
+ *            else xp = x (needs signal_len >= n_fft);  frames = 1 + (signal_len + (center ? n_fft : 0) - n_fft) / hop
+ *   inverse  the least-squares inverse, torch.istft(..., center, length = signal_len): every frame's irfft (normalised by 1/n_fft)
+ *            times the window, overlap-added, divided by the window envelope env[p] = sum_f w[p - f hop]^2, with the first
+ *            n_fft/2 samples dropped when center, and zeros past the last frame.  So inverse(forward(x)) = x.  This is the one
+ *            transform here that is normalised: the division by the envelope is part of what an inverse STFT is, and the 1/n_fft
+ *            folds into the same multiply (one table entry per sample, evaluated in long double and rounded once).  The
+ *            imaginary parts of bins 0 and n_fft/2 are ignored, as numpy's irfft ignores them.
+ * The inverse needs the NOLA condition, env > 1e-11 at every returned sample; it is checked at plan time in long double, and a plan
+ * that fails it (e.g. a periodic Hann window without center) runs its forward but returns B200FFT_ERR_UNSUPPORTED from the inverse.
+ * n_fft = 2^k with 4 <= n_fft <= 32768 (f64: 16384) runs the forward in one pass: one read of the signal and one write of the
+ * spectrum, no workspace.  Every other n_fft frames and windows into a workspace and runs the real plan of n_fft points from it
+ * (an n_fft whose real plan cannot be built is that plan's error); the inverse always runs the real plan's inverse into a workspace
+ * of whole rows of frames, then one overlap-add pass.  Workspaces come from the stream-ordered allocator (CUDA-graph capturable)
+ * in chunks of at most 2^27 reals (the inverse: at least one row).  signal_len and frames * n_fft must stay below 2^31
+ * (B200FFT_ERR_UNSUPPORTED).  Bad parameters and null pointers are B200FFT_ERR_INVALID_ARG.  Out of place only: overlapping input
+ * and output ranges are B200FFT_ERR_INVALID_ARG.  batch == 0 is a silent no-op.  Plans are immutable and thread safe; the device
+ * entry points are asynchronous on the stream. */
+typedef struct b200fft_stft_plan b200fft_stft_plan;
+int b200fft_stft_plan_create(b200fft_stft_plan** out, uint64_t signal_len, const void* window, uint64_t n_fft, uint64_t hop, int center,
+                             int precision, int device);
+int b200fft_stft_plan_destroy(b200fft_stft_plan* plan);
+/* e.g. "Stft{n=16000,n_fft=512,hop=128,center,frames=126,fused,M=256}",
+ * "Stft{n=16000,n_fft=400,hop=160,center,frames=101,rows=Real{Smooth{...}}}" (rows: the real plan's complex plan).  Returns length or <0. */
+int b200fft_stft_describe(const b200fft_stft_plan* plan, char* buf, uint64_t cap);
+/* Frames per row (0 for a NULL plan). */
+uint64_t b200fft_stft_frames(const b200fft_stft_plan* plan);
+/* d_signal: batch * signal_len reals, d_spectrum: batch * frames * (n_fft/2 + 1) complex values on the plan's device; asynchronous
+ * on `cuda_stream`. */
+int b200fft_stft_forward_device(const b200fft_stft_plan* plan, const void* d_signal, void* d_spectrum, uint64_t batch, void* cuda_stream);
+int b200fft_stft_inverse_device(const b200fft_stft_plan* plan, const void* d_spectrum, void* d_signal, uint64_t batch, void* cuda_stream);
+/* Same on host memory, synchronous (plain copies in and out, not pipelined). */
+int b200fft_stft_forward_host(const b200fft_stft_plan* plan, const void* signal, void* spectrum, uint64_t batch);
+int b200fft_stft_inverse_host(const b200fft_stft_plan* plan, const void* spectrum, void* signal, uint64_t batch);
+
 /* Message of the last failing call on this thread ("" if none). */
 const char* b200fft_last_error(void);
 /* Library build string: "b200fft <version> sm_90a" */

@@ -28,7 +28,7 @@ from typing import Dict, Optional, Tuple
 import numpy as np
 
 __all__ = ["FftDirection", "FftPlanner", "Fft", "Library", "FftError", "Recipe", "RealFftPlanner", "RealFft", "RealFft2d", "Fft2d", "FftConvolution",
-           "FftConvolution2d", "DctKind", "DctPlanner", "Dct", "DctNd",
+           "FftConvolution2d", "DctKind", "DctPlanner", "Dct", "DctNd", "Stft",
            "default_library", "shard_range"]
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -138,6 +138,8 @@ class Library:
         "b200fft_conv2d_device", "b200fft_conv2d_host",
         "b200fft_dct_plan_create", "b200fft_dct_plan_destroy", "b200fft_dct_describe", "b200fft_dct_device", "b200fft_dct_host",
         "b200fft_dctn_plan_create", "b200fft_dctn_plan_destroy", "b200fft_dctn_describe", "b200fft_dctn_device", "b200fft_dctn_host",
+        "b200fft_stft_plan_create", "b200fft_stft_plan_destroy", "b200fft_stft_describe", "b200fft_stft_frames",
+        "b200fft_stft_forward_device", "b200fft_stft_inverse_device", "b200fft_stft_forward_host", "b200fft_stft_inverse_host",
     ]
 
     def __init__(self, path: str = DEFAULT_LIB_PATH):
@@ -211,6 +213,15 @@ class Library:
         c.b200fft_dctn_describe.argtypes = [vp, ctypes.c_char_p, u64]
         c.b200fft_dctn_device.argtypes = [vp, vp, vp, u64, vp]
         c.b200fft_dctn_host.argtypes = [vp, vp, vp, u64]
+        c.b200fft_stft_plan_create.argtypes = [ctypes.POINTER(vp), u64, vp, u64, u64, i32, i32, i32]
+        c.b200fft_stft_plan_destroy.argtypes = [vp]
+        c.b200fft_stft_describe.argtypes = [vp, ctypes.c_char_p, u64]
+        c.b200fft_stft_frames.argtypes = [vp]
+        c.b200fft_stft_frames.restype = u64
+        c.b200fft_stft_forward_device.argtypes = [vp, vp, vp, u64, vp]
+        c.b200fft_stft_inverse_device.argtypes = [vp, vp, vp, u64, vp]
+        c.b200fft_stft_forward_host.argtypes = [vp, vp, vp, u64]
+        c.b200fft_stft_inverse_host.argtypes = [vp, vp, vp, u64]
 
     def device_count(self) -> int:
         n = ctypes.c_int(0)
@@ -651,6 +662,97 @@ class RealFftPlanner:
         """2-D convolution of real images of image_shape = (height, width) with the real 2-D `filter`; see FftConvolution2d (not
         cached: the filter is data)."""
         return FftConvolution2d(self._lib, filter, image_shape, mode, self._precision, self.device)
+
+    def plan_stft(self, window, hop: int, signal_len: int, center: bool = True) -> "Stft":
+        """Short-time Fourier transform of real rows of signal_len samples with the real 1-D `window` (its length is n_fft) and
+        `hop`; see Stft (not cached: the window is data)."""
+        return Stft(self._lib, window, hop, signal_len, center, self._precision, self.device)
+
+
+class Stft:
+    """Batched short-time Fourier transform of real rows with one window, hop, signal length and `center` fixed at plan time.
+    forward: batch * signal_len reals -> batch * frames * (n_fft/2 + 1) complex values, frame-major (row r, frame f, bin k at
+    (r frames + f) bins + k), unnormalised:
+
+        S[f][k] = sum_u w[u] xp[f hop + u] exp(-2 pi i k u / n_fft)
+
+    with xp the row reflect-padded by n_fft/2 on each side when center, so that S equals torch.stft(x, n_fft, hop, window=w,
+    center=center, pad_mode="reflect", return_complex=True).transpose(-2, -1).  inverse: the least-squares inverse, equal to
+    torch.istft(S.transpose(-2, -1), n_fft, hop, window=w, center=center, length=signal_len), so inverse(forward(x)) = x.  Unlike the
+    library's other transforms the inverse is normalised: the division by the window envelope sum_f w[t - f hop]^2 is part of an
+    inverse STFT, and the 1/n_fft folds into the same multiply.  It ignores the imaginary parts of bins 0 and n_fft/2, as numpy's
+    irfft does, and needs the NOLA condition (envelope > 1e-11 at every returned sample): a plan that fails it still runs forward,
+    and its inverse raises FftError (B200FFT_ERR_UNSUPPORTED).  Power-of-two n_fft from 4 to 32768 (f64: 16384) run the forward in
+    one pass; other even n_fft frame into a workspace and run the real plan.  Out of place only.  numpy arrays go through the
+    synchronous host entry points, torch CUDA tensors through the device ones (asynchronous on torch's current stream).  Immutable
+    and safe to call from many threads."""
+
+    def __init__(self, lib: Library, window, hop: int, signal_len: int, center: bool, precision: int, device: int):
+        self._lib, self._precision, self.device = lib, precision, device
+        self._hop, self._signal_len, self._center = int(hop), int(signal_len), bool(center)
+        if np.iscomplexobj(window):
+            raise TypeError("an STFT plan needs a real window")
+        w = np.ascontiguousarray(np.asarray(window), dtype=self.real_dtype)
+        if w.ndim != 1:
+            raise TypeError("the window must be 1-D")
+        self._n_fft = int(w.size)
+        self._h = ctypes.c_void_p()
+        lib.check(lib.c.b200fft_stft_plan_create(ctypes.byref(self._h), self._signal_len, w.ctypes.data, self._n_fft, self._hop,
+                                                 1 if self._center else 0, precision, device))
+        self._frames = int(lib.c.b200fft_stft_frames(self._h))
+
+    def __del__(self):
+        h, self._h = getattr(self, "_h", None), None
+        if h:
+            try:
+                self._lib.c.b200fft_stft_plan_destroy(h)
+            except Exception:
+                pass
+
+    @property
+    def real_dtype(self):
+        return np.float32 if self._precision == F32 else np.float64
+
+    @property
+    def complex_dtype(self):
+        return np.complex64 if self._precision == F32 else np.complex128
+
+    def n_fft(self) -> int:
+        return self._n_fft
+
+    def hop(self) -> int:
+        return self._hop
+
+    def signal_len(self) -> int:
+        return self._signal_len
+
+    def center(self) -> bool:
+        return self._center
+
+    def frames(self) -> int:
+        return self._frames
+
+    def bins(self) -> int:
+        return self._n_fft // 2 + 1
+
+    def describe(self) -> str:
+        buf = ctypes.create_string_buffer(512)
+        rc = self._lib.c.b200fft_stft_describe(self._h, buf, len(buf))
+        if rc < 0:
+            self._lib.check(rc)
+        return buf.value.decode()
+
+    def _run(self, inverse: bool, src, dst):
+        return _run_real(self._lib, self._h, self._precision, "Stft", "b200fft_stft", self._signal_len, self._frames * self.bins(), inverse,
+                         src, dst)
+
+    def forward(self, x, spec):
+        """Every row of `x` (batch * signal_len reals) into `spec` (batch * frames * bins complex values, any shape); returns `spec`."""
+        return self._run(False, x, spec)
+
+    def inverse(self, spec, y):
+        """Every row of spectra in `spec` (batch * frames * bins complex values) into `y` (batch * signal_len reals); returns `y`."""
+        return self._run(True, spec, y)
 
 
 class FftConvolution:
