@@ -332,6 +332,36 @@ int b200fft_stft_inverse_device(const b200fft_stft_plan* plan, const void* d_spe
 int b200fft_stft_forward_host(const b200fft_stft_plan* plan, const void* signal, void* spectrum, uint64_t batch);
 int b200fft_stft_inverse_host(const b200fft_stft_plan* plan, const void* spectrum, void* signal, uint64_t batch);
 
+/* Batched chirp-z transforms on the unit circle (scipy.signal.czt / zoom_fft).  For each contiguous row x of n samples and
+ * k = 0 .. m - 1:
+ *   y[k] = sum_{t<n} x[t] exp(-2 pi i (start + k step) t)     (unnormalised, like every transform here)
+ * with start and step in turns (cycles per sample): scipy.signal.czt(x, m, w = exp(-2 pi i step), a = exp(2 pi i start)), and
+ * zoom_fft(x, [f1, f2], m, fs, endpoint) is start = f1 / fs, step = (f2 - f1) / (fs m) (endpoint: / (fs (m - 1))).  start = 0,
+ * step = 1/n, m = n is the DFT; a negative step walks the circle backwards.  Only arcs of the unit circle: spirals (|a| != 1 or
+ * |w| != 1) are not supported.  The tables use the exact phase of the given doubles: start t + step t^2 / 2 is reduced mod 1 in
+ * 128-bit integers (to 2^-124 turns), evaluated in long double and rounded once, so that the error stays at FFT level up to
+ * n + m - 1 = 2^24 (forming w^(k^2/2) in double, as scipy does, loses accuracy as k^2 grows).
+ * domain B200FFT_CONV_COMPLEX: rows of complex samples; B200FFT_CONV_REAL: rows of reals (half the bytes read); the output is
+ * complex either way, batch * m values.  L = max(8, next_pow2(n + m - 1)) <= 4096 runs in one pass (Bluestein's fused kernel
+ * with the CZT's tables): one read of x and one write of y, no workspace.  8192 <= L <= 2^24 runs a pre-chirp pass, the L-point
+ * forward plan, a multiply pass, the L-point inverse plan and a post-chirp pass on a workspace from the stream-ordered allocator
+ * (CUDA-graph capturable), in chunks of whole rows of at most 2^27 complex values (one row at least).  n + m - 1 > 2^24 is
+ * B200FFT_ERR_UNSUPPORTED.  n = 0, m = 0, a start or step that is not finite, an unknown domain or precision, null pointers
+ * and overlapping input and output ranges are B200FFT_ERR_INVALID_ARG.  batch == 0 is a silent no-op.  Plans are immutable and
+ * thread safe; the device entry point is asynchronous on the stream. */
+typedef struct b200fft_czt_plan b200fft_czt_plan;
+int b200fft_czt_plan_create(b200fft_czt_plan** out, uint64_t n, uint64_t m, double start, double step, int domain, int precision,
+                            int device);
+int b200fft_czt_plan_destroy(b200fft_czt_plan* plan);
+/* e.g. "Czt{n=2000,m=1000,L=4096,real,fused}", "Czt{n=1000000,m=4096,L=1048576,complex,inner=FourStep{1024x1024}}" (inner: the
+ * L-point forward plan).  Returns length or <0. */
+int b200fft_czt_describe(const b200fft_czt_plan* plan, char* buf, uint64_t cap);
+/* d_in: batch * n samples (complex, or real for B200FFT_CONV_REAL), d_out: batch * m complex values, on the plan's device;
+ * asynchronous on `cuda_stream`. */
+int b200fft_czt_device(const b200fft_czt_plan* plan, const void* d_in, void* d_out, uint64_t batch, void* cuda_stream);
+/* Same on host memory, synchronous (plain copies in and out, not pipelined). */
+int b200fft_czt_host(const b200fft_czt_plan* plan, const void* in, void* out, uint64_t batch);
+
 /* Message of the last failing call on this thread ("" if none). */
 const char* b200fft_last_error(void);
 /* Library build string: "b200fft <version> sm_90a" */

@@ -28,7 +28,7 @@ from typing import Dict, Optional, Tuple
 import numpy as np
 
 __all__ = ["FftDirection", "FftPlanner", "Fft", "Library", "FftError", "Recipe", "RealFftPlanner", "RealFft", "RealFft2d", "Fft2d", "FftConvolution",
-           "FftConvolution2d", "DctKind", "DctPlanner", "Dct", "DctNd", "Stft",
+           "FftConvolution2d", "DctKind", "DctPlanner", "Dct", "DctNd", "Stft", "Czt",
            "default_library", "shard_range"]
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -140,6 +140,7 @@ class Library:
         "b200fft_dctn_plan_create", "b200fft_dctn_plan_destroy", "b200fft_dctn_describe", "b200fft_dctn_device", "b200fft_dctn_host",
         "b200fft_stft_plan_create", "b200fft_stft_plan_destroy", "b200fft_stft_describe", "b200fft_stft_frames",
         "b200fft_stft_forward_device", "b200fft_stft_inverse_device", "b200fft_stft_forward_host", "b200fft_stft_inverse_host",
+        "b200fft_czt_plan_create", "b200fft_czt_plan_destroy", "b200fft_czt_describe", "b200fft_czt_device", "b200fft_czt_host",
     ]
 
     def __init__(self, path: str = DEFAULT_LIB_PATH):
@@ -222,6 +223,11 @@ class Library:
         c.b200fft_stft_inverse_device.argtypes = [vp, vp, vp, u64, vp]
         c.b200fft_stft_forward_host.argtypes = [vp, vp, vp, u64]
         c.b200fft_stft_inverse_host.argtypes = [vp, vp, vp, u64]
+        c.b200fft_czt_plan_create.argtypes = [ctypes.POINTER(vp), u64, u64, ctypes.c_double, ctypes.c_double, i32, i32, i32]
+        c.b200fft_czt_plan_destroy.argtypes = [vp]
+        c.b200fft_czt_describe.argtypes = [vp, ctypes.c_char_p, u64]
+        c.b200fft_czt_device.argtypes = [vp, vp, vp, u64, vp]
+        c.b200fft_czt_host.argtypes = [vp, vp, vp, u64]
 
     def device_count(self) -> int:
         n = ctypes.c_int(0)
@@ -454,6 +460,18 @@ class FftPlanner:
         the filter is data)."""
         return FftConvolution(self._lib, filter, signal_len, mode, False, self._precision, self.device)
 
+
+    def plan_czt(self, n: int, m: Optional[int] = None, start: float = 0.0, step: Optional[float] = None) -> "Czt":
+        """Chirp-z transform of complex rows of n samples onto m points of the unit circle (default m = n), starting at `start` turns and
+        `step` turns apart (default 1/m, scipy's default w); see Czt (not cached)."""
+        m = int(n if m is None else m)
+        return Czt(self._lib, n, m, start, 1.0 / m if step is None else step, False, self._precision, self.device)
+
+    def plan_zoom_fft(self, n: int, fn, m: Optional[int] = None, fs: float = 2, endpoint: bool = False) -> "Czt":
+        """scipy.signal.ZoomFFT(n, fn, m, fs=fs, endpoint=endpoint) for complex rows: m points (default n) of the band fn = [f1, f2]
+        (a scalar fn is [0, fn]) of a signal sampled at fs; see Czt."""
+        return _zoom_fft(self, n, fn, m, fs, endpoint)
+
     def plan_fft_forward(self, len: int) -> Fft:
         return self.plan_fft(len, FftDirection.Forward)
 
@@ -668,6 +686,17 @@ class RealFftPlanner:
         `hop`; see Stft (not cached: the window is data)."""
         return Stft(self._lib, window, hop, signal_len, center, self._precision, self.device)
 
+    def plan_czt(self, n: int, m: Optional[int] = None, start: float = 0.0, step: Optional[float] = None) -> "Czt":
+        """Chirp-z transform of real rows of n samples onto m points of the unit circle (default m = n), starting at `start` turns and
+        `step` turns apart (default 1/m, scipy's default w); see Czt (not cached)."""
+        m = int(n if m is None else m)
+        return Czt(self._lib, n, m, start, 1.0 / m if step is None else step, True, self._precision, self.device)
+
+    def plan_zoom_fft(self, n: int, fn, m: Optional[int] = None, fs: float = 2, endpoint: bool = False) -> "Czt":
+        """scipy.signal.ZoomFFT(n, fn, m, fs=fs, endpoint=endpoint) for real rows: m points (default n) of the band fn = [f1, f2]
+        (a scalar fn is [0, fn]) of a signal sampled at fs; see Czt."""
+        return _zoom_fft(self, n, fn, m, fs, endpoint)
+
 
 class Stft:
     """Batched short-time Fourier transform of real rows with one window, hop, signal length and `center` fixed at plan time.
@@ -753,6 +782,113 @@ class Stft:
     def inverse(self, spec, y):
         """Every row of spectra in `spec` (batch * frames * bins complex values) into `y` (batch * signal_len reals); returns `y`."""
         return self._run(True, spec, y)
+
+
+def _zoom_fft(planner, n: int, fn, m: Optional[int], fs: float, endpoint: bool) -> "Czt":
+    f = np.atleast_1d(np.asarray(fn, dtype=np.float64))
+    if f.shape == (1,):
+        f1, f2 = 0.0, float(f[0])
+    elif f.shape == (2,):
+        f1, f2 = float(f[0]), float(f[1])
+    else:
+        raise ValueError("fn must be a scalar or a sequence of two frequencies [f1, f2]")
+    m = int(n if m is None else m)
+    if endpoint and m < 2:
+        raise ValueError("a zoom FFT with endpoint=True needs m >= 2 points")
+    return planner.plan_czt(n, m, f1 / fs, (f2 - f1) / (fs * (m - 1 if endpoint else m)))
+
+
+class Czt:
+    """Batched chirp-z transform on the unit circle with n, m, start and step fixed at plan time.  Every contiguous row x of n samples
+    becomes m complex values, unnormalised:
+
+        y[k] = sum_{t<n} x[t] exp(-2 pi i (start + k step) t),   k = 0 .. m - 1
+
+    with start and step in turns (cycles per sample).  This is scipy.signal.czt(x, m, w=exp(-2j pi step), a=exp(2j pi start)); a
+    caller holding scipy's unit-modulus w and a converts with step = -angle(w) / (2 pi) and start = angle(a) / (2 pi).  A zoom FFT
+    of the band [f1, f2] of a signal sampled at fs is start = f1 / fs, step = (f2 - f1) / (fs m) (endpoint: / (fs (m - 1))):
+    FftPlanner.plan_zoom_fft.  Spirals (|w| != 1 or |a| != 1) are not supported.  The tables use the exact phase of start and
+    step (reduced mod 1 in integers, not formed in double as scipy does), so the error stays at FFT level up to n + m - 1 = 2^24.
+
+    Complex rows from FftPlanner.plan_czt, real rows from RealFftPlanner.plan_czt (the output is complex either way).
+    max(8, next_pow2(n + m - 1)) <= 4096 runs in one pass (one read of x, one write of y); longer transforms run a pre-chirp pass,
+    the library's power-of-two forward and inverse plans and a post-chirp pass on a workspace.  Out of place only.  numpy arrays
+    go through the synchronous host entry point, torch CUDA tensors through the device one (asynchronous on torch's current
+    stream).  Immutable and safe to call from many threads."""
+
+    def __init__(self, lib: Library, n: int, m: int, start: float, step: float, real: bool, precision: int, device: int):
+        self._lib, self._real, self._precision, self.device = lib, bool(real), precision, device
+        self._n, self._m, self._start, self._step = int(n), int(m), float(start), float(step)
+        self._h = ctypes.c_void_p()
+        lib.check(lib.c.b200fft_czt_plan_create(ctypes.byref(self._h), self._n, self._m, self._start, self._step, 1 if real else 0,
+                                                precision, device))
+
+    def __del__(self):
+        h, self._h = getattr(self, "_h", None), None
+        if h:
+            try:
+                self._lib.c.b200fft_czt_plan_destroy(h)
+            except Exception:
+                pass
+
+    @property
+    def dtype(self):
+        """dtype of the input rows."""
+        if self._real:
+            return np.float32 if self._precision == F32 else np.float64
+        return self.out_dtype
+
+    @property
+    def out_dtype(self):
+        return np.complex64 if self._precision == F32 else np.complex128
+
+    def n(self) -> int:
+        return self._n
+
+    def m(self) -> int:
+        return self._m
+
+    def start(self) -> float:
+        return self._start
+
+    def step(self) -> float:
+        return self._step
+
+    def describe(self) -> str:
+        buf = ctypes.create_string_buffer(512)
+        rc = self._lib.c.b200fft_czt_describe(self._h, buf, len(buf))
+        if rc < 0:
+            self._lib.check(rc)
+        return buf.value.decode()
+
+    def _batch(self, n_in: int, n_out: int) -> int:
+        if n_in % self._n or n_out != n_in // self._n * self._m:
+            raise FftError(-6, f"Czt: input holds {n_in} samples, output {n_out}: expected batch * {self._n} and batch * {self._m}")
+        return n_in // self._n
+
+    def process(self, x, out):
+        """Transform every row of `x` (batch * n samples) into `out` (batch * m complex values, any shape); returns `out`."""
+        if isinstance(x, np.ndarray):
+            want, wout = np.dtype(self.dtype), np.dtype(self.out_dtype)
+            if not isinstance(out, np.ndarray) or x.dtype != want or out.dtype != wout or not x.flags.c_contiguous \
+                    or not out.flags.c_contiguous or not out.flags.writeable:
+                raise TypeError(f"Czt wants contiguous {want.name} input and a writable contiguous {wout.name} output")
+            batch = self._batch(x.size, out.size)
+            self._lib.check(self._lib.c.b200fft_czt_host(self._h, x.ctypes.data, out.ctypes.data, batch))
+            return out
+        import torch
+
+        tmap = {np.float32: torch.float32, np.float64: torch.float64, np.complex64: torch.complex64, np.complex128: torch.complex128}
+        want, wout = tmap[self.dtype], tmap[self.out_dtype]
+        if not isinstance(out, torch.Tensor) or x.dtype != want or out.dtype != wout or not x.is_cuda or not out.is_cuda \
+                or not x.is_contiguous() or not out.is_contiguous():
+            raise TypeError(f"Czt wants contiguous CUDA tensors of {want} (input) and {wout} (output)")
+        if x.device.index != self.device or out.device.index != self.device:
+            raise FftError(-1, f"tensors are on cuda:{x.device.index} / cuda:{out.device.index}, plan is on cuda:{self.device}")
+        batch = self._batch(x.numel(), out.numel())
+        self._lib.check(self._lib.c.b200fft_czt_device(self._h, x.data_ptr(), out.data_ptr(), batch,
+                                                       torch.cuda.current_stream(x.device).cuda_stream))
+        return out
 
 
 class FftConvolution:

@@ -175,6 +175,32 @@ template <typename T> B2_HD void st_stream(cx<T>* p, cx<T> v) {
     *p = v;
 #endif
 }
+// scalar forms of ld_stream / st_stream for real rows
+template <typename T> B2_HD T ld_stream_r(const T* p) {
+#if defined(__CUDA_ARCH__)
+    T r;
+    if constexpr (sizeof(T) == 4) {
+        asm volatile("ld.global.L1::no_allocate.L2::cache_hint.f32 %0, [%1], %2;" : "=f"(r) : "l"(p), "l"(l2_evict_first()));
+    } else {
+        asm volatile("ld.global.L1::no_allocate.L2::cache_hint.f64 %0, [%1], %2;" : "=d"(r) : "l"(p), "l"(l2_evict_first()));
+    }
+    return r;
+#else
+    return *p;
+#endif
+}
+template <typename T> B2_HD void st_stream_r(T* p, T v) {
+#if defined(__CUDA_ARCH__)
+    if constexpr (sizeof(T) == 4) {
+        asm volatile("st.global.L1::no_allocate.L2::cache_hint.f32 [%0], %1, %2;" ::"l"(p), "f"(v), "l"(l2_evict_first()) : "memory");
+    } else {
+        asm volatile("st.global.L1::no_allocate.L2::cache_hint.f64 [%0], %1, %2;" ::"l"(p), "d"(v), "l"(l2_evict_first()) : "memory");
+    }
+#else
+    *p = v;
+#endif
+}
+
 // "cache streaming" forms (ld/st.global.cs): what the four-step passes use.  Chosen by A/B timing:
 // the explicit no-allocate + L2-hint forms above are better for the one-pass Direct kernels, the .cs forms
 // for the two L2-coupled passes.

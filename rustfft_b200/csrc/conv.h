@@ -25,32 +25,6 @@
 
 namespace b2 {
 
-// scalar forms of ld_stream / st_stream (common.h) for real rows
-template <typename T> B2_HD T ld_stream_r(const T* p) {
-#if defined(__CUDA_ARCH__)
-    T r;
-    if constexpr (sizeof(T) == 4) {
-        asm volatile("ld.global.L1::no_allocate.L2::cache_hint.f32 %0, [%1], %2;" : "=f"(r) : "l"(p), "l"(l2_evict_first()));
-    } else {
-        asm volatile("ld.global.L1::no_allocate.L2::cache_hint.f64 %0, [%1], %2;" : "=d"(r) : "l"(p), "l"(l2_evict_first()));
-    }
-    return r;
-#else
-    return *p;
-#endif
-}
-template <typename T> B2_HD void st_stream_r(T* p, T v) {
-#if defined(__CUDA_ARCH__)
-    if constexpr (sizeof(T) == 4) {
-        asm volatile("st.global.L1::no_allocate.L2::cache_hint.f32 [%0], %1, %2;" ::"l"(p), "f"(v), "l"(l2_evict_first()) : "memory");
-    } else {
-        asm volatile("st.global.L1::no_allocate.L2::cache_hint.f64 [%0], %1, %2;" ::"l"(p), "d"(v), "l"(l2_evict_first()) : "memory");
-    }
-#else
-    *p = v;
-#endif
-}
-
 template <class G, bool REAL, int MINB = 1>
 struct OverlapSaveKernel {
     using T = typename G::T;

@@ -15,6 +15,18 @@ namespace hm {
 typedef long double ld;
 struct cld { ld x, y; };
 
+// cos / sin of the angle o pi/4 + (flip ? pi/4 - t : t), 0 <= t <= pi/4, from cosl / sinl of t
+inline void octant_sincos(unsigned o, bool flip, ld t, ld& c, ld& s) {
+    const ld ct = cosl(t), st = sinl(t);
+    const ld cphi = flip ? st : ct, sphi = flip ? ct : st;
+    switch (o >> 1) {
+        case 0: c = cphi; s = sphi; break;
+        case 1: c = -sphi; s = cphi; break;
+        case 2: c = -cphi; s = -sphi; break;
+        default: c = sphi; s = -cphi; break;
+    }
+}
+
 // cos(2*pi*k/n), sin(2*pi*k/n): integer octant reduction, then cosl/sinl on [0, pi/4].
 // Contract of src/twiddles.rs:6-23 (evaluate in higher precision, round once to T) -- here the
 // evaluation is 64-bit-mantissa long double with an exactly reduced argument.
@@ -26,14 +38,7 @@ inline void sincos_2pi(uint64_t k, uint64_t n, ld& c, ld& s) {
     const bool flip = (o & 1u) != 0;
     const ld quarter_pi = 0.785398163397448309615660845819875721L;
     const ld t = (flip ? (ld)(n - r) : (ld)r) / (ld)n * quarter_pi;
-    const ld ct = cosl(t), st = sinl(t);
-    const ld cphi = flip ? st : ct, sphi = flip ? ct : st;
-    switch (o >> 1) {
-        case 0: c = cphi; s = sphi; break;
-        case 1: c = -sphi; s = cphi; break;
-        case 2: c = -cphi; s = -sphi; break;
-        default: c = sphi; s = -cphi; break;
-    }
+    octant_sincos(o, flip, t, c, s);
 }
 
 // forward twiddle exp(-2*pi*i*k/n)
@@ -45,6 +50,42 @@ inline cld twiddle_ld(uint64_t k, uint64_t n) {
 template <typename T> inline cx<T> twiddle(uint64_t k, uint64_t n) {
     cld w = twiddle_ld(k, n);
     return mk<T>((T)w.x, (T)w.y);
+}
+
+// Phases of the chirp-z tables (impl.inl, czt_tables), in turns, reduced mod 1 exactly and kept as fixed-point fractions of
+// PHASE_BITS bits.  A finite double is m 2^e with |m| < 2^53, so v k for k < 2^62 (t^2 with t < 2^31) is the 115-bit integer m k
+// times a power of two: the integer turns drop out exactly, and only bits below 2^-124 turns are cut.  Evaluating the phase in
+// double instead would lose |v k| ulps of a turn, which grows with k^2 along a chirp.
+static constexpr int PHASE_BITS = 124;
+typedef unsigned __int128 u128;
+static constexpr u128 PHASE_ONE = (u128)1 << PHASE_BITS;
+// frac(v k 2^sh) in units of 2^-PHASE_BITS turns (v finite, k < 2^62, sh small)
+inline u128 frac_turns(double v, uint64_t k, int sh) {
+    if (v == 0 || k == 0) return 0;
+    int e;
+    const double fr = std::frexp(v, &e);
+    const int64_t m = (int64_t)std::ldexp(fr, 53);  // v = m 2^(e - 53), exactly
+    const int s = e - 53 + sh + PHASE_BITS;          // v k = (|m| k) 2^s units
+    const u128 a = (u128)(m < 0 ? -m : m) * k;
+    u128 r = 0;
+    if (s >= PHASE_BITS) r = 0;                       // whole turns
+    else if (s >= 0) r = (a << s) & (PHASE_ONE - 1);  // (mod 2^128, then mod 2^124: exact)
+    else if (s > -128) r = a >> -s;                   // below 2^-124 turns: cut
+    return m < 0 ? (PHASE_ONE - r) & (PHASE_ONE - 1) : r;
+}
+// exp(-2 pi i phase) for a phase of `num` units of 2^-PHASE_BITS turns: octant reduction on the integer, cosl / sinl on
+// [0, pi/4], one rounding to long double (the contract of sincos_2pi)
+inline cld turns_twiddle_ld(u128 num) {
+    num &= PHASE_ONE - 1;
+    const u128 eighth = PHASE_ONE >> 3;
+    const unsigned o = (unsigned)(num >> (PHASE_BITS - 3));
+    const u128 r = num & (eighth - 1);
+    const bool flip = (o & 1u) != 0;
+    const ld quarter_pi = 0.785398163397448309615660845819875721L;
+    const ld t = ldexpl((ld)(flip ? eighth - r : r), -(PHASE_BITS - 3)) * quarter_pi;
+    ld c, s;
+    octant_sincos(o, flip, t, c, s);
+    return cld{c, -s};
 }
 
 inline cld mul(cld a, cld b) { return cld{a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x}; }

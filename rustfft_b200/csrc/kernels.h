@@ -12,7 +12,8 @@
 //
 //   BluesteinKernel<G>   whole chirp-z transform of one signal in one CTA pass
 //                        (src/algorithm/bluesteins_algorithm.rs:100-136 fused: x*w -> FFT_M ->
-//                         *C, conj -> FFT_M -> conj * w)
+//                         *C, conj -> FFT_M -> conj * w; with separate input / output lengths and
+//                         tables it is the CZT of any arc on the unit circle)
 //   RaderKernel<G>       whole Rader transform of one prime-length signal in one CTA pass
 //                        (src/algorithm/raders_algorithm.rs:235-283 fused)
 //
@@ -461,10 +462,15 @@ struct FftKernel {
 };
 
 // ------------------------------------------------------------------------------------------
-// Bluestein, fully fused (M = G::L >= 2n-1).  chirp[i] = W_2n^(i^2 mod 2n) (src/twiddles.rs:25-57),
-// mult = FFT_M of the wrapped conjugate chirp / M (src/algorithm/bluesteins_algorithm.rs:62-83).
+// Chirp-z transform on the unit circle, fully fused (M = G::L >= n_in + n_out - 1):
+//   load x * pre (zero-padded to M) -> FFT_M -> * mult, conj -> FFT_M -> conj * post, first n_out
+// Bluestein's algorithm is the case n_in = n_out = n, pre = post = chirp[i] = W_2n^(i^2 mod 2n)
+// (src/twiddles.rs:25-57), mult = FFT_M of the wrapped conjugate chirp / M
+// (src/algorithm/bluesteins_algorithm.rs:62-83).  The CZT plans (impl.inl, czt_tables) fill the
+// same slots with the tables of an arbitrary arc.  REAL: the input rows are real (imaginary part 0;
+// half the bytes read), the output is complex.
 // ------------------------------------------------------------------------------------------
-template <class G, bool SWAP>
+template <class G, bool SWAP, bool REAL = false>
 struct BluesteinKernel {
     using T = typename G::T;
     using Eng = Engine<G, JF, JF>;
@@ -474,12 +480,13 @@ struct BluesteinKernel {
     static constexpr int NPHASE = 2 * NP1 - 1;
     static constexpr size_t SMEM_BYTES = sizeof(cx<T>) * (size_t)G::SMEM_ELEMS;
     struct Params {
-        const cx<T>* in;
-        cx<T>* out;
-        const cx<T>* chirp;  // n entries
+        const void* in;      // rows of n_in samples: cx<T>, or T when REAL
+        cx<T>* out;          // rows of n_out samples
+        const cx<T>* pre;    // n_in entries
+        const cx<T>* post;   // n_out entries
         const cx<T>* mult;   // M entries
         const cx<T>* tw;     // stage twiddles of the M-point FFT
-        uint32_t n;
+        uint32_t n_in, n_out;
         uint64_t n_fft;
     };
     struct Regs { cx<T> v[G::E]; };
@@ -491,15 +498,18 @@ struct BluesteinKernel {
         const uint64_t g = (uint64_t)bid * G::F + f;
         const bool ok = g < p.n_fft;
         if constexpr (P == 0) {
-            const cx<T>* src = p.in + g * (uint64_t)p.n;
             B2_UNROLL
             for (int q = 0; q < G::E; ++q) {
                 const uint32_t e = j + G::TP * q;
                 cx<T> v = mk<T>(0, 0);
-                if (ok && e < p.n) {
-                    v = ld_stream(src + e);
+                if (ok && e < p.n_in) {
+                    if constexpr (REAL) {
+                        v.x = ld_stream_r((const T*)p.in + g * (uint64_t)p.n_in + e);
+                    } else {
+                        v = ld_stream((const cx<T>*)p.in + g * (uint64_t)p.n_in + e);
+                    }
                     if (SWAP) v = swap_ri(v);
-                    v = cmul(v, ldg(p.chirp + e));
+                    v = cmul(v, ldg(p.pre + e));
                 }
                 r.v[q] = v;
             }
@@ -520,12 +530,12 @@ struct BluesteinKernel {
             Eng::template phase<P - NP1 + 1>(tid, r.v, smem, p.tw);
         }
         if constexpr (P == NPHASE - 1) {
-            cx<T>* dst = p.out + g * (uint64_t)p.n;
+            cx<T>* dst = p.out + g * (uint64_t)p.n_out;
             B2_UNROLL
             for (int q = 0; q < G::E; ++q) {
                 const uint32_t e = j + G::TP * q;
-                if (ok && e < p.n) {
-                    cx<T> v = cmul(conj(r.v[q]), ldg(p.chirp + e));
+                if (ok && e < p.n_out) {
+                    cx<T> v = cmul(conj(r.v[q]), ldg(p.post + e));
                     st_stream(dst + e, SWAP ? swap_ri(v) : v);
                 }
             }
