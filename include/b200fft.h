@@ -186,6 +186,48 @@ int b200fft_real2d_inverse_device(const b200fft_real_plan2d* plan, const void* d
 int b200fft_real2d_forward_host(const b200fft_real_plan2d* plan, const void* real_in, void* complex_out, uint64_t batch);
 int b200fft_real2d_inverse_host(const b200fft_real_plan2d* plan, const void* complex_in, void* real_out, uint64_t batch);
 
+/* 3-D complex transforms of row-major [depth][height][width] volumes (a batch of them, contiguous; numpy.fft.fftn over the last three
+ * axes, unnormalised, forward sign as everywhere here).  Replaces the caller's composition of b200fft_exec2d_* over the batch * D
+ * slices, a transpose that makes D the last axis, the D-point 1-D plan and a transpose back.  The width-point plan runs over every
+ * row (d_in -> d_out), then the H axis and the D axis each run in place on d_out, one pass per axis; an axis of length 1 is
+ * skipped.  An axis of length 2^k <= 4096 (f64: 2048) runs a compiled pass down the strided axis (one read and one write, no
+ * workspace); any other length <= 4096 (f64: 2048) with prime factors <= 31 runs the 2-D plans' column pass, which needs its
+ * columns fewer than 2^31 elements apart (H * W for the D axis); anything else is B200FFT_ERR_UNSUPPORTED, naming the axis.
+ * width: any length b200fft_plan_create accepts.  d_in == d_out (in place) is allowed, and out of place leaves the input intact;
+ * any other overlap is B200FFT_ERR_INVALID_ARG.  batch == 0 is a silent no-op.  Plans are immutable and thread safe; the device
+ * entry point is asynchronous on the stream (CUDA-graph capturable). */
+typedef struct b200fft_plan3d b200fft_plan3d;
+int b200fft_plan3d_create(b200fft_plan3d** out, uint64_t depth, uint64_t height, uint64_t width, int direction, int precision, int device);
+int b200fft_plan3d_destroy(b200fft_plan3d* plan);
+/* e.g. "Fft3d{256x256x256,rows=Direct{256},cols=Axis{256,F=16},depth=Axis{256,F=16}}", "...,cols=Columns{100 down [100x100]}"
+ * (rows: the width-point plan; cols: the H axis; depth: the D axis; absent when the axis has length 1).  Returns length or <0. */
+int b200fft_plan3d_describe(const b200fft_plan3d* plan, char* buf, uint64_t cap);
+/* d_in, d_out: batch * D * H * W complex values on the plan's device; asynchronous on `cuda_stream`. */
+int b200fft_exec3d_device(const b200fft_plan3d* plan, const void* d_in, void* d_out, uint64_t batch, void* cuda_stream);
+/* Same on host memory, synchronous (plain copies in and out, not pipelined). */
+int b200fft_exec3d_host(const b200fft_plan3d* plan, const void* in, void* out, uint64_t batch);
+
+/* 3-D real-input / real-output transforms of row-major [depth][height][width] real volumes (numpy.fft.rfftn / irfftn over the last
+ * three axes).  Replaces the caller's composition of b200fft_real2d_* over the batch * D slices with a transpose, the D-point
+ * complex plan and a transpose back.  forward: batch * D * H * W reals -> batch * D * H * (W/2 + 1) complex, unnormalised: the 2-D
+ * real transform of every [H][W] slice, then the D axis in place on the output.  inverse: the reverse, unnormalised, so
+ * inverse(forward(x)) = D * H * W * x; numpy's order (inverse complex transforms over D and H, then irfft over W), so for ANY half
+ * spectrum X it equals D * H * W * numpy.fft.irfftn(X, s=(D, H, W)).  The inverse runs the D axis out of place into a workspace of
+ * one spectrum's size from the stream-ordered allocator, then the 2-D real inverse from there: the input is never written.  depth 1
+ * is exactly b200fft_real_plan2d.  width and height follow b200fft_real_plan2d_create; depth follows the axis routes of
+ * b200fft_plan3d_create.  Out of place only: overlapping input and output ranges are B200FFT_ERR_INVALID_ARG.  batch == 0 is a
+ * silent no-op.  Plans are immutable and thread safe; the device entry points are asynchronous on the stream (CUDA-graph capturable). */
+typedef struct b200fft_real_plan3d b200fft_real_plan3d;
+int b200fft_real_plan3d_create(b200fft_real_plan3d** out, uint64_t depth, uint64_t height, uint64_t width, int precision, int device);
+int b200fft_real_plan3d_destroy(b200fft_real_plan3d* plan);
+/* e.g. "Real3d{64x64x64,plane=Real2d{64x64,rows=Direct{32}},depth=Axis{64,F=32}}".  Returns length or <0. */
+int b200fft_real_plan3d_describe(const b200fft_real_plan3d* plan, char* buf, uint64_t cap);
+int b200fft_real3d_forward_device(const b200fft_real_plan3d* plan, const void* d_real_in, void* d_complex_out, uint64_t batch, void* cuda_stream);
+int b200fft_real3d_inverse_device(const b200fft_real_plan3d* plan, const void* d_complex_in, void* d_real_out, uint64_t batch, void* cuda_stream);
+/* Same on host memory, synchronous (plain copies in and out, not pipelined). */
+int b200fft_real3d_forward_host(const b200fft_real_plan3d* plan, const void* real_in, void* complex_out, uint64_t batch);
+int b200fft_real3d_inverse_host(const b200fft_real_plan3d* plan, const void* complex_in, void* real_out, uint64_t batch);
+
 /* Batched FFT convolution (SURVEY 8(f).4; what scipy.signal.fftconvolve / oaconvolve do): every row of a batch of rows of
  * signal_len samples, contiguous, is convolved with ONE filter of filter_len taps fixed at plan time.  Plain sums, no scaling;
  * the result equals scipy.signal.fftconvolve(row, filter, mode):

@@ -141,6 +141,9 @@ class Library:
         "b200fft_stft_plan_create", "b200fft_stft_plan_destroy", "b200fft_stft_describe", "b200fft_stft_frames",
         "b200fft_stft_forward_device", "b200fft_stft_inverse_device", "b200fft_stft_forward_host", "b200fft_stft_inverse_host",
         "b200fft_czt_plan_create", "b200fft_czt_plan_destroy", "b200fft_czt_describe", "b200fft_czt_device", "b200fft_czt_host",
+        "b200fft_plan3d_create", "b200fft_plan3d_destroy", "b200fft_plan3d_describe", "b200fft_exec3d_device", "b200fft_exec3d_host",
+        "b200fft_real_plan3d_create", "b200fft_real_plan3d_destroy", "b200fft_real_plan3d_describe", "b200fft_real3d_forward_device",
+        "b200fft_real3d_inverse_device", "b200fft_real3d_forward_host", "b200fft_real3d_inverse_host",
     ]
 
     def __init__(self, path: str = DEFAULT_LIB_PATH):
@@ -228,6 +231,18 @@ class Library:
         c.b200fft_czt_describe.argtypes = [vp, ctypes.c_char_p, u64]
         c.b200fft_czt_device.argtypes = [vp, vp, vp, u64, vp]
         c.b200fft_czt_host.argtypes = [vp, vp, vp, u64]
+        c.b200fft_plan3d_create.argtypes = [ctypes.POINTER(vp), u64, u64, u64, i32, i32, i32]
+        c.b200fft_plan3d_destroy.argtypes = [vp]
+        c.b200fft_plan3d_describe.argtypes = [vp, ctypes.c_char_p, u64]
+        c.b200fft_exec3d_device.argtypes = [vp, vp, vp, u64, vp]
+        c.b200fft_exec3d_host.argtypes = [vp, vp, vp, u64]
+        c.b200fft_real_plan3d_create.argtypes = [ctypes.POINTER(vp), u64, u64, u64, i32, i32]
+        c.b200fft_real_plan3d_destroy.argtypes = [vp]
+        c.b200fft_real_plan3d_describe.argtypes = [vp, ctypes.c_char_p, u64]
+        c.b200fft_real3d_forward_device.argtypes = [vp, vp, vp, u64, vp]
+        c.b200fft_real3d_inverse_device.argtypes = [vp, vp, vp, u64, vp]
+        c.b200fft_real3d_forward_host.argtypes = [vp, vp, vp, u64]
+        c.b200fft_real3d_inverse_host.argtypes = [vp, vp, vp, u64]
 
     def device_count(self) -> int:
         n = ctypes.c_int(0)
@@ -455,6 +470,11 @@ class FftPlanner:
         """2-D transform of [height][width] images: the width-point plan over the rows, one strided pass down the columns."""
         return Fft2d(self._lib, height, width, direction, self._precision, self.device)
 
+    def plan_fft_3d(self, depth: int, height: int, width: int, direction: FftDirection = FftDirection.Forward) -> "Fft3d":
+        """3-D transform of [depth][height][width] volumes: the width-point plan over the rows, then one strided pass down each of
+        the other two axes (not cached, like plan_fft_2d)."""
+        return Fft3d(self._lib, depth, height, width, direction, self._precision, self.device)
+
     def plan_convolution(self, filter, signal_len: int, mode: str = "full") -> "FftConvolution":
         """Convolution of complex rows of signal_len samples with `filter` (1-D, 1..2048 taps); see FftConvolution (not cached:
         the filter is data)."""
@@ -521,6 +541,65 @@ class Fft2d:
         if x.numel() % per:
             raise FftError(-5, f"Input FFT buffer must be a multiple of FFT length. Expected multiple of {per}, got len = {x.numel()}")
         self._lib.check(self._lib.c.b200fft_exec2d_device(self._h, x.data_ptr(), dst.data_ptr(), x.numel() // per,
+                                                          torch.cuda.current_stream(x.device).cuda_stream))
+        return dst
+
+
+class Fft3d:
+    """3-D complex transform of row-major [depth][height][width] volumes (a batch of them, contiguous): numpy.fft.fftn over the last
+    three axes, unnormalised, forward sign as in 1-D.  The width-point plan runs over the rows, then one pass down the H axis and one
+    down the D axis: a compiled strided pass for power-of-two lengths up to 4096 (f64: 2048), the 2-D plans' column pass for other
+    31-smooth lengths.  numpy arrays go through the synchronous host entry point (in place), torch CUDA tensors through the device one
+    (in place or into `out`, asynchronous on torch's current stream).  Immutable and safe to call from many threads."""
+
+    def __init__(self, lib: Library, depth: int, height: int, width: int, direction: FftDirection, precision: int, device: int):
+        self._lib, self._precision, self.device = lib, precision, device
+        self._shape = (int(depth), int(height), int(width))
+        self._direction = FftDirection(direction)
+        self._h = ctypes.c_void_p()
+        lib.check(lib.c.b200fft_plan3d_create(ctypes.byref(self._h), *self._shape, int(direction), precision, device))
+
+    def __del__(self):
+        h, self._h = getattr(self, "_h", None), None
+        if h:
+            try:
+                self._lib.c.b200fft_plan3d_destroy(h)
+            except Exception:
+                pass
+
+    def fft_direction(self) -> FftDirection:
+        return self._direction
+
+    def shape(self) -> Tuple[int, int, int]:
+        return self._shape
+
+    def describe(self) -> str:
+        buf = ctypes.create_string_buffer(1024)
+        rc = self._lib.c.b200fft_plan3d_describe(self._h, buf, len(buf))
+        if rc < 0:
+            self._lib.check(rc)
+        return buf.value.decode()
+
+    def process(self, buffer: np.ndarray) -> None:
+        want = np.complex64 if self._precision == F32 else np.complex128
+        if not isinstance(buffer, np.ndarray) or buffer.dtype != want or not buffer.flags.c_contiguous or not buffer.flags.writeable:
+            raise TypeError(f"Fft3d.process wants a contiguous writable {np.dtype(want)} array")
+        per = self._shape[0] * self._shape[1] * self._shape[2]
+        if buffer.size % per:
+            raise FftError(-5, f"Input FFT buffer must be a multiple of FFT length. Expected multiple of {per}, got len = {buffer.size}")
+        self._lib.check(self._lib.c.b200fft_exec3d_host(self._h, buffer.ctypes.data, buffer.ctypes.data, buffer.size // per))
+
+    def process_device(self, x, out=None):
+        import torch
+
+        want = torch.complex64 if self._precision == F32 else torch.complex128
+        dst = x if out is None else out
+        if x.dtype != want or dst.dtype != want or not x.is_cuda or not x.is_contiguous() or not dst.is_contiguous() or dst.numel() != x.numel():
+            raise TypeError(f"Fft3d.process_device wants contiguous CUDA tensors of {want} with equal sizes")
+        per = self._shape[0] * self._shape[1] * self._shape[2]
+        if x.numel() % per:
+            raise FftError(-5, f"Input FFT buffer must be a multiple of FFT length. Expected multiple of {per}, got len = {x.numel()}")
+        self._lib.check(self._lib.c.b200fft_exec3d_device(self._h, x.data_ptr(), dst.data_ptr(), x.numel() // per,
                                                           torch.cuda.current_stream(x.device).cuda_stream))
         return dst
 
@@ -636,6 +715,60 @@ class RealFft2d:
         return self._run(True, complex_in, real_out)
 
 
+class RealFft3d:
+    """3-D real-to-complex / complex-to-real transforms of row-major [depth][height][width] real volumes (a batch of them, contiguous),
+    even width: numpy.fft.rfftn / irfftn over the last three axes.  forward: batch * D * H * W reals -> batch * D * H * (W/2 + 1)
+    complex, unnormalised; inverse: the reverse, unnormalised (inverse(forward(x)) == D * H * W * x), equal to
+    D * H * W * numpy.fft.irfftn(X, s=(D, H, W)) for any half spectrum X.  The 2-D real transform of every [H][W] slice, then one pass
+    down the D axis (the inverse: the D axis into a workspace first, so the input is never written); depth 1 is exactly RealFft2d.
+    Out of place only.  numpy arrays go through the synchronous host entry points, torch CUDA tensors through the device ones
+    (asynchronous on torch's current stream).  Immutable and safe to call from many threads."""
+
+    def __init__(self, lib: Library, depth: int, height: int, width: int, precision: int, device: int):
+        self._lib, self._precision, self.device = lib, precision, device
+        self._depth, self._height, self._width = int(depth), int(height), int(width)
+        self._h = ctypes.c_void_p()
+        lib.check(lib.c.b200fft_real_plan3d_create(ctypes.byref(self._h), self._depth, self._height, self._width, precision, device))
+
+    def __del__(self):
+        h, self._h = getattr(self, "_h", None), None
+        if h:
+            try:
+                self._lib.c.b200fft_real_plan3d_destroy(h)
+            except Exception:
+                pass
+
+    def depth(self) -> int:
+        return self._depth
+
+    def height(self) -> int:
+        return self._height
+
+    def width(self) -> int:
+        return self._width
+
+    def complex_width(self) -> int:
+        return self._width // 2 + 1
+
+    def describe(self) -> str:
+        buf = ctypes.create_string_buffer(1024)
+        rc = self._lib.c.b200fft_real_plan3d_describe(self._h, buf, len(buf))
+        if rc < 0:
+            self._lib.check(rc)
+        return buf.value.decode()
+
+    def _run(self, inverse: bool, src, dst):
+        dh = self._depth * self._height
+        return _run_real(self._lib, self._h, self._precision, "RealFft3d", "b200fft_real3d", dh * self._width, dh * self.complex_width(),
+                         inverse, src, dst)
+
+    def forward(self, real_in, complex_out):
+        return self._run(False, real_in, complex_out)
+
+    def inverse(self, complex_in, real_out):
+        return self._run(True, complex_in, real_out)
+
+
 class RealFftPlanner:
     """Plans RealFft instances (cached per length), like realfft::RealFftPlanner over rustfft::FftPlanner."""
 
@@ -653,6 +786,7 @@ class RealFftPlanner:
         self.device = device
         self._cache: Dict[int, RealFft] = {}
         self._cache_2d: Dict[Tuple[int, int], RealFft2d] = {}
+        self._cache_3d: Dict[Tuple[int, int, int], RealFft3d] = {}
         self._lock = threading.Lock()
 
     def plan_fft(self, len: int) -> RealFft:
@@ -669,6 +803,15 @@ class RealFftPlanner:
             f = self._cache_2d.get(key)
             if f is None:
                 f = self._cache_2d[key] = RealFft2d(self._lib, key[0], key[1], self._precision, self.device)
+            return f
+
+    def plan_fft_3d(self, depth: int, height: int, width: int) -> RealFft3d:
+        """3-D real transform of [depth][height][width] volumes (even width), cached per shape; see RealFft3d."""
+        key = (int(depth), int(height), int(width))
+        with self._lock:
+            f = self._cache_3d.get(key)
+            if f is None:
+                f = self._cache_3d[key] = RealFft3d(self._lib, key[0], key[1], key[2], self._precision, self.device)
             return f
 
     def plan_convolution(self, filter, signal_len: int, mode: str = "full") -> FftConvolution:

@@ -1,0 +1,4 @@
+// libb200fft.so -- the f64 compiled axis pass of the 3-D plans (AxisKernel, fft3d.h), in a translation unit of its own.
+#include "rt_cuda.h"
+#define B2_PART_FFT3D64 1
+#include "impl.inl"
