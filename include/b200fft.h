@@ -255,6 +255,32 @@ int b200fft_conv_device(const b200fft_conv_plan* plan, const void* d_in, void* d
 /* Same on host memory, synchronous (plain copies in and out, not pipelined). */
 int b200fft_conv_host(const b200fft_conv_plan* plan, const void* in, void* out, uint64_t batch);
 
+/* Batched multi-channel FFT convolution: C filters of filter_len taps each (host memory, row-major [C][filter_len], fixed at plan
+ * time), every output row convolved with its own filter.  Modes, domains, output lengths and filter limits as for b200fft_conv_*;
+ * plain sums, no scaling.  The output is batch * C rows of output_len samples, row (b, c) at (b C + c) output_len.  Layouts:
+ *   PER_CHANNEL  input batch * C rows of signal_len samples, row (b, c) at (b C + c) signal_len:  y[b][c] = x[b][c] (*) h[c]
+ *                = scipy.signal.fftconvolve(x, h[None], mode, axes=-1) for x of shape [batch][C][signal_len]
+ *   SHARED       input batch rows, a filter bank over each:  y[b][c] = x[b] (*) h[c]
+ *                = scipy.signal.fftconvolve(x[:, None, :], h[None], mode, axes=-1) for "full" and "valid" (for "same", scipy crops
+ *                the channel axis to x's: broadcast x to [batch][C][signal_len] first)
+ * One launch and one pass over device memory per call, like the single-filter plans; the C spectra stay on the device with the
+ * plan.  C = 1 is exactly the b200fft_conv plan.  channels == 0 is B200FFT_ERR_INVALID_ARG; spectrum tables above 2^31 bytes are
+ * B200FFT_ERR_UNSUPPORTED.  Out of place only.  signal_len == 0 or batch == 0 is a silent no-op.  Immutable and thread safe. */
+typedef struct b200fft_chconv_plan b200fft_chconv_plan;
+enum { B200FFT_CHCONV_PER_CHANNEL = 0, B200FFT_CHCONV_SHARED = 1 };
+int b200fft_chconv_plan_create(b200fft_chconv_plan** out, uint64_t signal_len, uint64_t channels, const void* filters, uint64_t filter_len,
+                               int mode, int domain, int layout, int precision, int device);
+int b200fft_chconv_plan_destroy(b200fft_chconv_plan* plan);
+/* Samples per output row (0 for a NULL plan). */
+uint64_t b200fft_chconv_output_len(const b200fft_chconv_plan* plan);
+/* e.g. "ChannelOverlapSave{n=65536,m=255,C=64,M=2048,L=1794,full,real,per_channel}".  Returns length or <0. */
+int b200fft_chconv_describe(const b200fft_chconv_plan* plan, char* buf, uint64_t cap);
+/* d_in: batch * C * signal_len samples (SHARED: batch * signal_len), d_out: batch * C * output_len samples, on the plan's device;
+ * asynchronous on `cuda_stream`. */
+int b200fft_chconv_device(const b200fft_chconv_plan* plan, const void* d_in, void* d_out, uint64_t batch, void* cuda_stream);
+/* Same on host memory, synchronous (plain copies in and out, not pipelined). */
+int b200fft_chconv_host(const b200fft_chconv_plan* plan, const void* in, void* out, uint64_t batch);
+
 /* Batched 2-D FFT convolution of real images: every [height][width] image of a batch of real images (row-major, contiguous) is
  * convolved with ONE real filter of [filter_height][filter_width] taps (row-major, host memory) fixed at plan time.  Plain sums,
  * no scaling; the result equals scipy.signal.fftconvolve(image, filter, mode) in 2-D, with the B200FFT_CONV_* modes per axis:

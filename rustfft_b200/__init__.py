@@ -28,7 +28,7 @@ from typing import Dict, Optional, Tuple
 import numpy as np
 
 __all__ = ["FftDirection", "FftPlanner", "Fft", "Library", "FftError", "Recipe", "RealFftPlanner", "RealFft", "RealFft2d", "Fft2d", "FftConvolution",
-           "FftConvolution2d", "DctKind", "DctPlanner", "Dct", "DctNd", "Stft", "Czt",
+           "ChannelConvolution", "FftConvolution2d", "DctKind", "DctPlanner", "Dct", "DctNd", "Stft", "Czt",
            "default_library", "shard_range"]
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -132,6 +132,8 @@ class Library:
         "b200fft_plan2d_create", "b200fft_plan2d_destroy", "b200fft_exec2d_device", "b200fft_exec2d_host",
         "b200fft_conv_plan_create", "b200fft_conv_plan_destroy", "b200fft_conv_output_len", "b200fft_conv_describe",
         "b200fft_conv_device", "b200fft_conv_host",
+        "b200fft_chconv_plan_create", "b200fft_chconv_plan_destroy", "b200fft_chconv_output_len", "b200fft_chconv_describe",
+        "b200fft_chconv_device", "b200fft_chconv_host",
         "b200fft_real_plan2d_create", "b200fft_real_plan2d_destroy", "b200fft_real_plan2d_describe", "b200fft_real2d_forward_device",
         "b200fft_real2d_inverse_device", "b200fft_real2d_forward_host", "b200fft_real2d_inverse_host",
         "b200fft_conv2d_plan_create", "b200fft_conv2d_plan_destroy", "b200fft_conv2d_output_shape", "b200fft_conv2d_describe",
@@ -194,6 +196,13 @@ class Library:
         c.b200fft_conv_describe.argtypes = [vp, ctypes.c_char_p, u64]
         c.b200fft_conv_device.argtypes = [vp, vp, vp, u64, vp]
         c.b200fft_conv_host.argtypes = [vp, vp, vp, u64]
+        c.b200fft_chconv_plan_create.argtypes = [ctypes.POINTER(vp), u64, u64, vp, u64, i32, i32, i32, i32, i32]
+        c.b200fft_chconv_plan_destroy.argtypes = [vp]
+        c.b200fft_chconv_output_len.argtypes = [vp]
+        c.b200fft_chconv_output_len.restype = u64
+        c.b200fft_chconv_describe.argtypes = [vp, ctypes.c_char_p, u64]
+        c.b200fft_chconv_device.argtypes = [vp, vp, vp, u64, vp]
+        c.b200fft_chconv_host.argtypes = [vp, vp, vp, u64]
         c.b200fft_real_plan2d_create.argtypes = [ctypes.POINTER(vp), u64, u64, i32, i32]
         c.b200fft_real_plan2d_destroy.argtypes = [vp]
         c.b200fft_real_plan2d_describe.argtypes = [vp, ctypes.c_char_p, u64]
@@ -479,6 +488,12 @@ class FftPlanner:
         """Convolution of complex rows of signal_len samples with `filter` (1-D, 1..2048 taps); see FftConvolution (not cached:
         the filter is data)."""
         return FftConvolution(self._lib, filter, signal_len, mode, False, self._precision, self.device)
+
+    def plan_channel_convolution(self, filters, signal_len: int, mode: str = "full", shared_input: bool = False) -> "ChannelConvolution":
+        """Convolution of complex rows with one of C complex filters each (`filters`: [C][m], 1..2048 taps; 1-D is C = 1): per
+        channel, or a filter bank over shared input rows when shared_input; see ChannelConvolution (not cached: the filters are
+        data)."""
+        return ChannelConvolution(self._lib, filters, signal_len, mode, shared_input, False, self._precision, self.device)
 
 
     def plan_czt(self, n: int, m: Optional[int] = None, start: float = 0.0, step: Optional[float] = None) -> "Czt":
@@ -819,6 +834,11 @@ class RealFftPlanner:
         cached: the filter is data)."""
         return FftConvolution(self._lib, filter, signal_len, mode, True, self._precision, self.device)
 
+    def plan_channel_convolution(self, filters, signal_len: int, mode: str = "full", shared_input: bool = False) -> "ChannelConvolution":
+        """Convolution of real rows with one of C real filters each (`filters`: [C][m], 1..2048 taps; 1-D is C = 1): per channel, or
+        a filter bank over shared input rows when shared_input; see ChannelConvolution (not cached: the filters are data)."""
+        return ChannelConvolution(self._lib, filters, signal_len, mode, shared_input, True, self._precision, self.device)
+
     def plan_convolution_2d(self, filter, image_shape, mode: str = "full") -> "FftConvolution2d":
         """2-D convolution of real images of image_shape = (height, width) with the real 2-D `filter`; see FftConvolution2d (not
         cached: the filter is data)."""
@@ -1119,6 +1139,108 @@ class FftConvolution:
         batch = self._batch(x.numel(), out.numel())
         self._lib.check(self._lib.c.b200fft_conv_device(self._h, x.data_ptr(), out.data_ptr(), batch,
                                                         torch.cuda.current_stream(x.device).cuda_stream))
+        return out
+
+
+class ChannelConvolution:
+    """Batched multi-channel FFT convolution with C filters of m taps fixed at plan time.  The output is batch * C rows of
+    output_len samples, row (b, c) at (b C + c) output_len, and every row is scipy.signal.fftconvolve(input row, filters[c], mode)
+    -- plain sums, no scaling, modes and output lengths as for FftConvolution:
+      per channel (default)  input [batch][C][signal_len]:  y[b][c] = x[b][c] (*) h[c]
+                             = scipy.signal.fftconvolve(x, h[None], mode, axes=-1)
+      shared_input=True      input [batch][signal_len], a filter bank over each row:  y[b][c] = x[b] (*) h[c]
+                             = scipy.signal.fftconvolve(np.broadcast_to(x[:, None, :], (batch, C, signal_len)), h[None], mode,
+                             axes=-1)  (without the broadcast, scipy's "same" crops the channel axis to 1)
+    Complex rows and filters from FftPlanner.plan_channel_convolution, real ones from RealFftPlanner.plan_channel_convolution.
+    C = 1 (a 1-D filters array) computes exactly what FftConvolution does.
+
+    One launch and one pass over device memory (overlap-save inside one CTA per block), out of place only.  numpy arrays go
+    through the synchronous host entry point, torch CUDA tensors through the device one (asynchronous on torch's current
+    stream).  Immutable and safe to call from many threads."""
+
+    MODES = FftConvolution.MODES
+
+    def __init__(self, lib: Library, filters, signal_len: int, mode: str, shared: bool, real: bool, precision: int, device: int):
+        if mode not in self.MODES:
+            raise FftError(-1, f"unknown convolution mode {mode!r}: expected one of {sorted(self.MODES)}")
+        self._lib, self._real, self._precision, self.device, self.mode = lib, bool(real), precision, device, mode
+        self._shared, self._signal_len = bool(shared), int(signal_len)
+        if real and np.iscomplexobj(filters):
+            raise TypeError("a real convolution plan needs real filters")
+        h = np.ascontiguousarray(np.asarray(filters), dtype=self.dtype)
+        if h.ndim == 1:
+            h = h[None]
+        if h.ndim != 2:
+            raise TypeError("the filters must be 1-D or 2-D ([channels][taps])")
+        self._channels = int(h.shape[0])
+        self._h = ctypes.c_void_p()
+        lib.check(lib.c.b200fft_chconv_plan_create(ctypes.byref(self._h), self._signal_len, self._channels, h.ctypes.data, h.shape[1],
+                                                   self.MODES[mode], 1 if real else 0, 1 if shared else 0, precision, device))
+        self._out_len = int(lib.c.b200fft_chconv_output_len(self._h))
+
+    def __del__(self):
+        h, self._h = getattr(self, "_h", None), None
+        if h:
+            try:
+                self._lib.c.b200fft_chconv_plan_destroy(h)
+            except Exception:
+                pass
+
+    @property
+    def dtype(self):
+        if self._real:
+            return np.float32 if self._precision == F32 else np.float64
+        return np.complex64 if self._precision == F32 else np.complex128
+
+    def channels(self) -> int:
+        return self._channels
+
+    def signal_len(self) -> int:
+        return self._signal_len
+
+    def output_len(self) -> int:
+        return self._out_len
+
+    def describe(self) -> str:
+        buf = ctypes.create_string_buffer(256)
+        rc = self._lib.c.b200fft_chconv_describe(self._h, buf, len(buf))
+        if rc < 0:
+            self._lib.check(rc)
+        return buf.value.decode()
+
+    def _batch(self, n_in: int, n_out: int) -> int:
+        C, o = self._channels, self._out_len
+        n = self._signal_len * (1 if self._shared else C)  # input samples per batch element
+        if n == 0:
+            return 0
+        if n_in % n or n_out != n_in // n * C * o:
+            raise FftError(-6, f"ChannelConvolution: input holds {n_in} samples, output {n_out}: expected batch * {n} and "
+                               f"batch * {C * o}")
+        return n_in // n
+
+    def process(self, x, out):
+        """Convolve every input row of `x` (batch * C * signal_len samples, or batch * signal_len with shared input) into `out`
+        (batch * C * output_len samples); returns `out`."""
+        if isinstance(x, np.ndarray):
+            want = np.dtype(self.dtype)
+            if not isinstance(out, np.ndarray) or x.dtype != want or out.dtype != want or not x.flags.c_contiguous \
+                    or not out.flags.c_contiguous or not out.flags.writeable:
+                raise TypeError(f"ChannelConvolution wants contiguous {want.name} input and a writable {want.name} output")
+            batch = self._batch(x.size, out.size)
+            self._lib.check(self._lib.c.b200fft_chconv_host(self._h, x.ctypes.data, out.ctypes.data, batch))
+            return out
+        import torch
+
+        tmap = {np.float32: torch.float32, np.float64: torch.float64, np.complex64: torch.complex64, np.complex128: torch.complex128}
+        want = tmap[self.dtype]
+        if not isinstance(out, torch.Tensor) or x.dtype != want or out.dtype != want or not x.is_cuda or not out.is_cuda \
+                or not x.is_contiguous() or not out.is_contiguous():
+            raise TypeError(f"ChannelConvolution wants contiguous CUDA tensors of {want}")
+        if x.device.index != self.device or out.device.index != self.device:
+            raise FftError(-1, f"tensors are on cuda:{x.device.index} / cuda:{out.device.index}, plan is on cuda:{self.device}")
+        batch = self._batch(x.numel(), out.numel())
+        self._lib.check(self._lib.c.b200fft_chconv_device(self._h, x.data_ptr(), out.data_ptr(), batch,
+                                                          torch.cuda.current_stream(x.device).cuda_stream))
         return out
 
 
