@@ -430,6 +430,31 @@ int b200fft_czt_device(const b200fft_czt_plan* plan, const void* d_in, void* d_o
 /* Same on host memory, synchronous (plain copies in and out, not pipelined). */
 int b200fft_czt_host(const b200fft_czt_plan* plan, const void* in, void* out, uint64_t batch);
 
+/* Batched analytic signals of real rows (scipy.signal.hilbert(x, axis=-1)).  For each contiguous row x of N reals the output row
+ * is N complex values z = x + i y:
+ *   y[n] = sum_m x[m] (2/N) sum_{0<k<N/2} sin(2 pi k (n - m) / N)
+ * that is ifft(fft(x) h) with h = 1, 2, ..., 2, (1 at N/2 for even N), 0, ...  The analytic signal is normalised by definition:
+ * unlike the library's FFTs, the real part is x, copied bit for bit on every path.  N = 1 gives z = x; N = 0 plans and every
+ * call is a silent no-op.  Power-of-two N from 4 to 32768 (f64: 16384) run in one pass: one read of x, one write of z, no
+ * workspace.  Other even N run the N/2-point forward plan on x read as complex pairs, a pass on the spectrum and the N/2-point
+ * inverse plan on a workspace from the stream-ordered allocator (CUDA-graph capturable), in chunks of whole rows of at most 2^27
+ * complex values (one row at least), then a pass that writes z.  Odd N run in the output buffer itself (x promoted to complex, the
+ * N-point forward plan, a sign multiply, the N-point inverse plan, x written into the real parts).  A length whose complex plan
+ * (N/2 points for even N, N for odd N) this build cannot make is B200FFT_ERR_UNSUPPORTED.  Even N read x as pairs: a device
+ * input that does not start at an even element is B200FFT_ERR_INVALID_ARG, as are an unknown precision, null pointers and
+ * overlapping input and output ranges (out of place only).  batch == 0 is a silent no-op.  Plans are immutable and thread safe;
+ * the device entry point is asynchronous on the stream. */
+typedef struct b200fft_hilbert_plan b200fft_hilbert_plan;
+int b200fft_hilbert_plan_create(b200fft_hilbert_plan** out, uint64_t len, int precision, int device);
+int b200fft_hilbert_plan_destroy(b200fft_hilbert_plan* plan);
+/* e.g. "Hilbert{n=4096,fused,M=2048}", "Hilbert{n=48000,inner=SmoothFourStep{64x375,compiled}}" (inner: the forward complex plan), "Hilbert{n=1,identity}",
+ * "Hilbert{n=0,empty}".  Returns length or <0. */
+int b200fft_hilbert_describe(const b200fft_hilbert_plan* plan, char* buf, uint64_t cap);
+/* d_in: batch * len reals, d_out: batch * len complex values, on the plan's device; asynchronous on `cuda_stream`. */
+int b200fft_hilbert_device(const b200fft_hilbert_plan* plan, const void* d_in, void* d_out, uint64_t batch, void* cuda_stream);
+/* Same on host memory, synchronous (plain copies in and out, not pipelined). */
+int b200fft_hilbert_host(const b200fft_hilbert_plan* plan, const void* in, void* out, uint64_t batch);
+
 /* Message of the last failing call on this thread ("" if none). */
 const char* b200fft_last_error(void);
 /* Library build string: "b200fft <version> sm_90a" */

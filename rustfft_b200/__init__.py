@@ -28,7 +28,7 @@ from typing import Dict, Optional, Tuple
 import numpy as np
 
 __all__ = ["FftDirection", "FftPlanner", "Fft", "Library", "FftError", "Recipe", "RealFftPlanner", "RealFft", "RealFft2d", "Fft2d", "FftConvolution",
-           "ChannelConvolution", "FftConvolution2d", "DctKind", "DctPlanner", "Dct", "DctNd", "Stft", "Czt",
+           "ChannelConvolution", "FftConvolution2d", "DctKind", "DctPlanner", "Dct", "DctNd", "Stft", "Czt", "Hilbert",
            "default_library", "shard_range"]
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -143,6 +143,8 @@ class Library:
         "b200fft_stft_plan_create", "b200fft_stft_plan_destroy", "b200fft_stft_describe", "b200fft_stft_frames",
         "b200fft_stft_forward_device", "b200fft_stft_inverse_device", "b200fft_stft_forward_host", "b200fft_stft_inverse_host",
         "b200fft_czt_plan_create", "b200fft_czt_plan_destroy", "b200fft_czt_describe", "b200fft_czt_device", "b200fft_czt_host",
+        "b200fft_hilbert_plan_create", "b200fft_hilbert_plan_destroy", "b200fft_hilbert_describe", "b200fft_hilbert_device",
+        "b200fft_hilbert_host",
         "b200fft_plan3d_create", "b200fft_plan3d_destroy", "b200fft_plan3d_describe", "b200fft_exec3d_device", "b200fft_exec3d_host",
         "b200fft_real_plan3d_create", "b200fft_real_plan3d_destroy", "b200fft_real_plan3d_describe", "b200fft_real3d_forward_device",
         "b200fft_real3d_inverse_device", "b200fft_real3d_forward_host", "b200fft_real3d_inverse_host",
@@ -240,6 +242,11 @@ class Library:
         c.b200fft_czt_describe.argtypes = [vp, ctypes.c_char_p, u64]
         c.b200fft_czt_device.argtypes = [vp, vp, vp, u64, vp]
         c.b200fft_czt_host.argtypes = [vp, vp, vp, u64]
+        c.b200fft_hilbert_plan_create.argtypes = [ctypes.POINTER(vp), u64, i32, i32]
+        c.b200fft_hilbert_plan_destroy.argtypes = [vp]
+        c.b200fft_hilbert_describe.argtypes = [vp, ctypes.c_char_p, u64]
+        c.b200fft_hilbert_device.argtypes = [vp, vp, vp, u64, vp]
+        c.b200fft_hilbert_host.argtypes = [vp, vp, vp, u64]
         c.b200fft_plan3d_create.argtypes = [ctypes.POINTER(vp), u64, u64, u64, i32, i32, i32]
         c.b200fft_plan3d_destroy.argtypes = [vp]
         c.b200fft_plan3d_describe.argtypes = [vp, ctypes.c_char_p, u64]
@@ -802,6 +809,7 @@ class RealFftPlanner:
         self._cache: Dict[int, RealFft] = {}
         self._cache_2d: Dict[Tuple[int, int], RealFft2d] = {}
         self._cache_3d: Dict[Tuple[int, int, int], RealFft3d] = {}
+        self._cache_hilbert: Dict[int, Hilbert] = {}
         self._lock = threading.Lock()
 
     def plan_fft(self, len: int) -> RealFft:
@@ -828,6 +836,14 @@ class RealFftPlanner:
             if f is None:
                 f = self._cache_3d[key] = RealFft3d(self._lib, key[0], key[1], key[2], self._precision, self.device)
             return f
+
+    def plan_hilbert(self, len: int) -> "Hilbert":
+        """Analytic signal (scipy.signal.hilbert) of real rows of `len` samples, cached per length; see Hilbert."""
+        with self._lock:
+            h = self._cache_hilbert.get(int(len))
+            if h is None:
+                h = self._cache_hilbert[int(len)] = Hilbert(self._lib, int(len), self._precision, self.device)
+            return h
 
     def plan_convolution(self, filter, signal_len: int, mode: str = "full") -> FftConvolution:
         """Convolution of real rows of signal_len samples with the real `filter` (1-D, 1..2048 taps); see FftConvolution (not
@@ -1051,6 +1067,83 @@ class Czt:
         batch = self._batch(x.numel(), out.numel())
         self._lib.check(self._lib.c.b200fft_czt_device(self._h, x.data_ptr(), out.data_ptr(), batch,
                                                        torch.cuda.current_stream(x.device).cuda_stream))
+        return out
+
+
+class Hilbert:
+    """Batched analytic signal of real rows, scipy.signal.hilbert(x, axis=-1): every contiguous row x of len() reals becomes len()
+    complex values z = x + i y, with y the Hilbert transform of x,
+
+        z = ifft(fft(x) h),   h = 1, 2, ..., 2, (1 at N/2 for even N), 0, ...
+
+    Normalised, unlike the library's FFTs: the real part of z is x itself, bit for bit.  |z| is the envelope and angle(z) the
+    instantaneous phase.  Power-of-two lengths from 4 to 32768 (f64: 16384) run in one pass (one read of x, one write of z); other
+    even lengths run the len/2-point complex plans on a workspace, odd lengths the len-point plans in the output itself.  Even
+    lengths read x as pairs, so a CUDA tensor input must start at an even element (TypeError otherwise).  Out of place only.  numpy
+    arrays go through the synchronous host entry point, torch CUDA tensors through the device one (asynchronous on torch's
+    current stream).  From RealFftPlanner.plan_hilbert.  Immutable and safe to call from many threads."""
+
+    def __init__(self, lib: Library, length: int, precision: int, device: int):
+        self._lib, self._len, self._precision, self.device = lib, int(length), precision, device
+        self._h = ctypes.c_void_p()
+        lib.check(lib.c.b200fft_hilbert_plan_create(ctypes.byref(self._h), self._len, precision, device))
+
+    def __del__(self):
+        h, self._h = getattr(self, "_h", None), None
+        if h:
+            try:
+                self._lib.c.b200fft_hilbert_plan_destroy(h)
+            except Exception:
+                pass
+
+    def len(self) -> int:
+        return self._len
+
+    @property
+    def dtype(self):
+        """dtype of the input rows."""
+        return np.float32 if self._precision == F32 else np.float64
+
+    @property
+    def out_dtype(self):
+        return np.complex64 if self._precision == F32 else np.complex128
+
+    def describe(self) -> str:
+        buf = ctypes.create_string_buffer(512)
+        rc = self._lib.c.b200fft_hilbert_describe(self._h, buf, len(buf))
+        if rc < 0:
+            self._lib.check(rc)
+        return buf.value.decode()
+
+    def _batch(self, n_in: int, n_out: int) -> int:
+        if n_in != n_out or (self._len and n_in % self._len) or (not self._len and n_in):
+            raise FftError(-6, f"Hilbert: input holds {n_in} samples, output {n_out}: expected batch * {self._len} each")
+        return n_in // self._len if self._len else 0
+
+    def process(self, x, out):
+        """Every row of `x` (batch * len() reals) into `out` (batch * len() complex values, any shape); returns `out`."""
+        if isinstance(x, np.ndarray):
+            want, wout = np.dtype(self.dtype), np.dtype(self.out_dtype)
+            if not isinstance(out, np.ndarray) or x.dtype != want or out.dtype != wout or not x.flags.c_contiguous \
+                    or not out.flags.c_contiguous or not out.flags.writeable:
+                raise TypeError(f"Hilbert wants contiguous {want.name} input and a writable contiguous {wout.name} output")
+            batch = self._batch(x.size, out.size)
+            self._lib.check(self._lib.c.b200fft_hilbert_host(self._h, x.ctypes.data, out.ctypes.data, batch))
+            return out
+        import torch
+
+        want = torch.float32 if self._precision == F32 else torch.float64
+        wout = torch.complex64 if self._precision == F32 else torch.complex128
+        if not isinstance(out, torch.Tensor) or x.dtype != want or out.dtype != wout or not x.is_cuda or not out.is_cuda \
+                or not x.is_contiguous() or not out.is_contiguous():
+            raise TypeError(f"Hilbert wants contiguous CUDA tensors of {want} (input) and {wout} (output)")
+        if x.device.index != self.device or out.device.index != self.device:
+            raise FftError(-1, f"tensors are on cuda:{x.device.index} / cuda:{out.device.index}, plan is on cuda:{self.device}")
+        if self._len % 2 == 0 and x.data_ptr() % (2 * x.element_size()):
+            raise TypeError("Hilbert.process: even lengths read x as pairs, so the input tensor must start at an even element")
+        batch = self._batch(x.numel(), out.numel())
+        self._lib.check(self._lib.c.b200fft_hilbert_device(self._h, x.data_ptr(), out.data_ptr(), batch,
+                                                           torch.cuda.current_stream(x.device).cuda_stream))
         return out
 
 
