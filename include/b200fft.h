@@ -455,6 +455,44 @@ int b200fft_hilbert_device(const b200fft_hilbert_plan* plan, const void* d_in, v
 /* Same on host memory, synchronous (plain copies in and out, not pipelined). */
 int b200fft_hilbert_host(const b200fft_hilbert_plan* plan, const void* in, void* out, uint64_t batch);
 
+/* Batched modified DCTs of real rows (rustdct's Mdct).  A plan fixes N = len (even, >= 2), a real `window` of 2N taps (host memory,
+ * in the plan's precision; any values) and signal_len L >= 1.  A row x is padded as xp = N zeros, x, zeros up to (frames + 1) N
+ * samples, frames = ceil(L / N) + 1, and frame f covers xp[f N, f N + 2N).  A signal buffer holds batch contiguous rows of L reals; a
+ * coefficient buffer holds batch * frames * N reals, frame-major: row r, frame f, coefficient k at (r frames + f) N + k.
+ *   forward  C[f][k] = sum_{n<2N} w[n] xp[f N + n] cos(pi/N (n + 1/2 + N/2)(k + 1/2)),  k < N   (unnormalised, as rustdct defines
+ *            it: row f is rustdct's process_mdct(xp[fN .. fN+N], xp[fN+N .. fN+2N]))
+ *   inverse  y = (2/N) sum_f w[n] sum_k C[f][k] cos(pi/N (n + 1/2 + N/2)(k + 1/2)) placed at f N + n and overlap-added, cropped to
+ *            [N, N + L): the sum of rustdct's process_imdct outputs times 2/N.  If w[n]^2 + w[n+N]^2 = 1 and w[2N-1-n] = w[n]
+ *            (sine, Vorbis, KBD windows) then inverse(forward(x)) = x, the first and last N samples included.  Any other window
+ *            computes the same formula (no envelope division).  The 2/N folds into one window table entry per tap, evaluated in long
+ *            double and rounded once.
+ * N = 2^k with 64 <= N <= 512 (f64: 64 <= N <= 16384) runs the forward in one pass: the quarter fold of the windowed frames, then the
+ * N-point DCT-IV, one read of the signal and one write of the coefficients, no workspace (the lengths where that pass beat the
+ * general route on an H100; README).  Every other even N folds into the coefficient
+ * buffer and runs the N-point Dct4 plan on it in place (the environment variable B200FFT_MDCT_ROUTE=general, read once per process,
+ * sends power-of-two N down this route too).  The inverse runs the Dct4 plan from the coefficients into a workspace of whole rows
+ * of frames (stream-ordered allocator, CUDA-graph capturable; chunks of at most 2^27 reals, one row at least), then one overlap-add
+ * pass.  Odd N is B200FFT_ERR_UNSUPPORTED (the fold needs N/2); so are L >= 2^31 and frames * N >= 2^31.  An N whose Dct4 plan
+ * cannot be built is that plan's error.  len = 0, L = 0, an unknown precision, null pointers and overlapping input and output ranges
+ * (out of place only) are B200FFT_ERR_INVALID_ARG, and so is a coefficient buffer that does not start at an even element when the
+ * N-point Dct4 is a one-pass plan (the power-of-two N above: the fused passes move coefficient pairs).  The signal buffer takes any
+ * offset.  batch == 0 is a silent no-op.  Plans are immutable and thread safe; the device entry points are asynchronous on the
+ * stream. */
+typedef struct b200fft_mdct_plan b200fft_mdct_plan;
+int b200fft_mdct_plan_create(b200fft_mdct_plan** out, uint64_t len, const void* window, uint64_t signal_len, int precision, int device);
+int b200fft_mdct_plan_destroy(b200fft_mdct_plan* plan);
+/* e.g. "Mdct{n=512,L=48000,frames=95,fused,M=256}", "Mdct{n=960,L=48000,frames=51,dct=Dct4{n=960,inner=...}}" (dct: the N-point
+ * Dct4 plan of the general forward).  Returns length or <0. */
+int b200fft_mdct_describe(const b200fft_mdct_plan* plan, char* buf, uint64_t cap);
+/* Frames per row (0 for a NULL plan). */
+uint64_t b200fft_mdct_frames(const b200fft_mdct_plan* plan);
+/* d_signal: batch * signal_len reals, d_coefs: batch * frames * len reals on the plan's device; asynchronous on `cuda_stream`. */
+int b200fft_mdct_forward_device(const b200fft_mdct_plan* plan, const void* d_signal, void* d_coefs, uint64_t batch, void* cuda_stream);
+int b200fft_mdct_inverse_device(const b200fft_mdct_plan* plan, const void* d_coefs, void* d_signal, uint64_t batch, void* cuda_stream);
+/* Same on host memory, synchronous (plain copies in and out, not pipelined). */
+int b200fft_mdct_forward_host(const b200fft_mdct_plan* plan, const void* signal, void* coefs, uint64_t batch);
+int b200fft_mdct_inverse_host(const b200fft_mdct_plan* plan, const void* coefs, void* signal, uint64_t batch);
+
 /* Message of the last failing call on this thread ("" if none). */
 const char* b200fft_last_error(void);
 /* Library build string: "b200fft <version> sm_90a" */

@@ -168,3 +168,97 @@ impl<T> Drop for CudaDctNd<T> {
         unsafe { b200fft_dctn_plan_destroy(self.plan) };
     }
 }
+
+#[repr(C)]
+pub struct B200FftMdctPlan {
+    _private: [u8; 0],
+}
+
+#[link(name = "b200fft")]
+extern "C" {
+    fn b200fft_mdct_plan_create(out: *mut *mut B200FftMdctPlan, len: u64, window: *const c_void, signal_len: u64, precision: c_int,
+                                device: c_int) -> c_int;
+    fn b200fft_mdct_plan_destroy(plan: *mut B200FftMdctPlan) -> c_int;
+    fn b200fft_mdct_describe(plan: *const B200FftMdctPlan, buf: *mut c_char, cap: u64) -> c_int;
+    fn b200fft_mdct_frames(plan: *const B200FftMdctPlan) -> u64;
+    fn b200fft_mdct_forward_host(plan: *const B200FftMdctPlan, signal: *const c_void, coefs: *mut c_void, batch: u64) -> c_int;
+    fn b200fft_mdct_inverse_host(plan: *const B200FftMdctPlan, coefs: *const c_void, signal: *mut c_void, batch: u64) -> c_int;
+}
+
+/// One planned MDCT (rustdct's `Mdct`, from `plan_mdct(len, window_fn)`) over whole signal rows of `signal_len` samples.
+///
+/// Frame mapping: a row x is padded as xp = `len` zeros, x, zeros, and cut into `frames()` = ceil(signal_len / len) + 1 frames of
+/// 2 len samples at a hop of len.  Row f of `forward`'s output (frame-major, `frames()` rows of len coefficients per signal row) is
+/// rustdct's `process_mdct(&xp[f len .. f len + len], &xp[f len + len .. f len + 2 len], &mut row)`.  `inverse` is the
+/// overlap-add of rustdct's `process_imdct(&row_f, ...)` over the frames, placed at f len, times 2 / len, cropped to
+/// [len, len + signal_len): with a Princen-Bradley window (sine, Vorbis, KBD) `inverse(forward(x)) = x`.  The window has 2 len taps
+/// (rustdct's `window_fn::sine` / `vorbis` evaluated by the caller).  `Sync + Send`: the plan handle is immutable.
+pub struct CudaMdct<T> {
+    plan: *mut B200FftMdctPlan,
+    len: usize,
+    signal_len: usize,
+    frames: usize,
+    _t: PhantomData<T>,
+}
+unsafe impl<T> Send for CudaMdct<T> {}
+unsafe impl<T> Sync for CudaMdct<T> {}
+
+impl<T: FftNum> CudaMdct<T> {
+    pub fn new(len: usize, window: &[T], signal_len: usize) -> Result<Self, String> {
+        let precision = if TypeId::of::<T>() == TypeId::of::<f32>() { 0 } else if TypeId::of::<T>() == TypeId::of::<f64>() { 1 } else {
+            return Err("CudaMdct supports f32 and f64 only".into());
+        };
+        if window.len() != 2 * len {
+            return Err(format!("an MDCT of len {} needs a window of {} taps (got {})", len, 2 * len, window.len()));
+        }
+        let mut plan = std::ptr::null_mut();
+        let rc = unsafe { b200fft_mdct_plan_create(&mut plan, len as u64, window.as_ptr().cast(), signal_len as u64, precision, 0) };
+        if rc != 0 {
+            return Err(super::last_error_text());
+        }
+        let frames = unsafe { b200fft_mdct_frames(plan) } as usize;
+        Ok(Self { plan, len, signal_len, frames, _t: PhantomData })
+    }
+    pub fn len(&self) -> usize {
+        self.len
+    }
+    pub fn frames(&self) -> usize {
+        self.frames
+    }
+    pub fn describe(&self) -> String {
+        let mut buf = vec![0u8; 512];
+        let n = unsafe { b200fft_mdct_describe(self.plan, buf.as_mut_ptr().cast(), buf.len() as u64) };
+        if n < 0 {
+            return String::new();
+        }
+        buf.truncate(n as usize);
+        String::from_utf8_lossy(&buf).into_owned()
+    }
+    /// Every row of `signal` (batch * signal_len samples) into `coefs` (batch * frames() * len()).  Panics with the library's message.
+    pub fn forward(&self, signal: &[T], coefs: &mut [T]) {
+        assert!(signal.len() % self.signal_len == 0, "Mdct: signal holds {} samples, expected a multiple of {}", signal.len(), self.signal_len);
+        let batch = signal.len() / self.signal_len;
+        assert_eq!(coefs.len(), batch * self.frames * self.len, "Mdct: coefficient buffer of the wrong size");
+        let rc = unsafe { b200fft_mdct_forward_host(self.plan, signal.as_ptr().cast(), coefs.as_mut_ptr().cast(), batch as u64) };
+        if rc != 0 {
+            panic!("{}", super::last_error_text());
+        }
+    }
+    /// Every row of `coefs` (batch * frames() * len()) into `signal` (batch * signal_len samples).  Panics with the library's message.
+    pub fn inverse(&self, coefs: &[T], signal: &mut [T]) {
+        let per = self.frames * self.len;
+        assert!(coefs.len() % per == 0, "Mdct: coefficient buffer holds {} values, expected a multiple of {}", coefs.len(), per);
+        let batch = coefs.len() / per;
+        assert_eq!(signal.len(), batch * self.signal_len, "Mdct: signal buffer of the wrong size");
+        let rc = unsafe { b200fft_mdct_inverse_host(self.plan, coefs.as_ptr().cast(), signal.as_mut_ptr().cast(), batch as u64) };
+        if rc != 0 {
+            panic!("{}", super::last_error_text());
+        }
+    }
+}
+
+impl<T> Drop for CudaMdct<T> {
+    fn drop(&mut self) {
+        unsafe { b200fft_mdct_plan_destroy(self.plan) };
+    }
+}

@@ -28,7 +28,7 @@ from typing import Dict, Optional, Tuple
 import numpy as np
 
 __all__ = ["FftDirection", "FftPlanner", "Fft", "Library", "FftError", "Recipe", "RealFftPlanner", "RealFft", "RealFft2d", "Fft2d", "FftConvolution",
-           "ChannelConvolution", "FftConvolution2d", "DctKind", "DctPlanner", "Dct", "DctNd", "Stft", "Czt", "Hilbert",
+           "ChannelConvolution", "FftConvolution2d", "DctKind", "DctPlanner", "Dct", "DctNd", "Stft", "Czt", "Hilbert", "Mdct", "mdct_window",
            "default_library", "shard_range"]
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -145,6 +145,8 @@ class Library:
         "b200fft_czt_plan_create", "b200fft_czt_plan_destroy", "b200fft_czt_describe", "b200fft_czt_device", "b200fft_czt_host",
         "b200fft_hilbert_plan_create", "b200fft_hilbert_plan_destroy", "b200fft_hilbert_describe", "b200fft_hilbert_device",
         "b200fft_hilbert_host",
+        "b200fft_mdct_plan_create", "b200fft_mdct_plan_destroy", "b200fft_mdct_describe", "b200fft_mdct_frames",
+        "b200fft_mdct_forward_device", "b200fft_mdct_inverse_device", "b200fft_mdct_forward_host", "b200fft_mdct_inverse_host",
         "b200fft_plan3d_create", "b200fft_plan3d_destroy", "b200fft_plan3d_describe", "b200fft_exec3d_device", "b200fft_exec3d_host",
         "b200fft_real_plan3d_create", "b200fft_real_plan3d_destroy", "b200fft_real_plan3d_describe", "b200fft_real3d_forward_device",
         "b200fft_real3d_inverse_device", "b200fft_real3d_forward_host", "b200fft_real3d_inverse_host",
@@ -247,6 +249,15 @@ class Library:
         c.b200fft_hilbert_describe.argtypes = [vp, ctypes.c_char_p, u64]
         c.b200fft_hilbert_device.argtypes = [vp, vp, vp, u64, vp]
         c.b200fft_hilbert_host.argtypes = [vp, vp, vp, u64]
+        c.b200fft_mdct_plan_create.argtypes = [ctypes.POINTER(vp), u64, vp, u64, i32, i32]
+        c.b200fft_mdct_plan_destroy.argtypes = [vp]
+        c.b200fft_mdct_describe.argtypes = [vp, ctypes.c_char_p, u64]
+        c.b200fft_mdct_frames.argtypes = [vp]
+        c.b200fft_mdct_frames.restype = u64
+        c.b200fft_mdct_forward_device.argtypes = [vp, vp, vp, u64, vp]
+        c.b200fft_mdct_inverse_device.argtypes = [vp, vp, vp, u64, vp]
+        c.b200fft_mdct_forward_host.argtypes = [vp, vp, vp, u64]
+        c.b200fft_mdct_inverse_host.argtypes = [vp, vp, vp, u64]
         c.b200fft_plan3d_create.argtypes = [ctypes.POINTER(vp), u64, u64, u64, i32, i32, i32]
         c.b200fft_plan3d_destroy.argtypes = [vp]
         c.b200fft_plan3d_describe.argtypes = [vp, ctypes.c_char_p, u64]
@@ -1522,6 +1533,132 @@ class Dct:
         return dst
 
 
+_PI_LD = np.longdouble("3.14159265358979323846264338327950288")
+
+
+def mdct_window(name: str, length: int, dtype=np.float64) -> np.ndarray:
+    """rustdct's window_fn::sine / vorbis of 2 * length taps, evaluated in np.longdouble and rounded once to `dtype`:
+    sine[n] = sin(pi (n + 1/2) / 2N), vorbis[n] = sin(pi/2 sin^2(pi (n + 1/2) / 2N))."""
+    n = np.arange(2 * int(length), dtype=np.longdouble)
+    s = np.sin(_PI_LD * (n + np.longdouble(0.5)) / np.longdouble(2 * int(length)))
+    if name == "sine":
+        return s.astype(dtype)
+    if name == "vorbis":
+        return np.sin(_PI_LD / 2 * s * s).astype(dtype)
+    raise ValueError(f"unknown MDCT window {name!r}: expected 'sine', 'vorbis' or an array of 2 * len taps")
+
+
+class Mdct:
+    """Batched modified DCT of real rows (rustdct's Mdct) with N = len(), a real window w of 2N taps and the signal length L fixed at
+    plan time.  A row x is padded with N zeros on each side and cut into frames() = ceil(L / N) + 1 frames of 2N samples at a hop of
+    N; frame f covers xp[f N, f N + 2N), xp = N zeros, x, zeros.  forward: batch * L reals -> batch * frames * N reals, frame-major,
+    unnormalised as rustdct defines it:
+
+        C[f][k] = sum_{n < 2N} w[n] xp[f N + n] cos(pi/N (n + 1/2 + N/2)(k + 1/2))
+
+    so row f equals rustdct's process_mdct(xp[fN .. fN + N], xp[fN + N .. fN + 2N]).  inverse: the overlap-add of (2/N) times
+    rustdct's process_imdct of every frame, cropped to [N, N + L).  For a Princen-Bradley window (w[n]^2 + w[n + N]^2 = 1,
+    w[2N - 1 - n] = w[n]: "sine", "vorbis", KBD) inverse(forward(x)) = x, the first and last N samples included; any other window
+    computes the same formula.  N must be even.  Power-of-two N from 64 to 512 (f64: 64 to 16384) run the forward in one pass (the
+    lengths where that pass beat the general route on an H100); other N fold into the output and run the N-point Dct4 plan on it.  The inverse runs the Dct4 plan into a workspace, then one overlap-add pass.
+    When the Dct4 of N is a one-pass plan the coefficient tensor must start at an even element (TypeError otherwise).  Out of place
+    only.  numpy arrays go through the synchronous host entry points (forward / inverse), torch CUDA tensors through the device ones
+    (forward_device / inverse_device, asynchronous on torch's current stream).  From DctPlanner.plan_mdct.  Immutable and safe to
+    call from many threads."""
+
+    def __init__(self, lib: Library, length: int, window: np.ndarray, signal_len: int, precision: int, device: int):
+        self._lib, self._len, self._signal_len, self._precision, self.device = lib, int(length), int(signal_len), precision, device
+        self._h = ctypes.c_void_p()
+        lib.check(lib.c.b200fft_mdct_plan_create(ctypes.byref(self._h), self._len, window.ctypes.data, self._signal_len, precision, device))
+        self._frames = int(lib.c.b200fft_mdct_frames(self._h))
+        self._pairs = re.search(r"(^Mdct\{[^{]*|dct=Dct4\{n=\d+),fused,", self.describe()) is not None
+
+    def __del__(self):
+        h, self._h = getattr(self, "_h", None), None
+        if h:
+            try:
+                self._lib.c.b200fft_mdct_plan_destroy(h)
+            except Exception:
+                pass
+
+    def len(self) -> int:
+        return self._len
+
+    def signal_len(self) -> int:
+        return self._signal_len
+
+    def frames(self) -> int:
+        return self._frames
+
+    @property
+    def dtype(self):
+        return np.float32 if self._precision == F32 else np.float64
+
+    def describe(self) -> str:
+        buf = ctypes.create_string_buffer(1024)
+        rc = self._lib.c.b200fft_mdct_describe(self._h, buf, len(buf))
+        if rc < 0:
+            self._lib.check(rc)
+        return buf.value.decode()
+
+    def _host(self, kind: str, src, dst, sper: int, dper: int):
+        want = np.dtype(self.dtype)
+        if not isinstance(src, np.ndarray) or src.dtype != want or not src.flags.c_contiguous:
+            raise TypeError(f"Mdct.{kind} wants a contiguous {want.name} array")
+        if src.size % sper:
+            raise FftError(-6, f"Mdct: input holds {src.size} elements, expected batch * {sper}")
+        batch = src.size // sper
+        if dst is None:
+            dst = np.empty((batch, self._frames, self._len) if kind == "forward" else (batch, self._signal_len), want)
+        if not isinstance(dst, np.ndarray) or dst.dtype != want or not dst.flags.c_contiguous or not dst.flags.writeable:
+            raise TypeError(f"Mdct.{kind} wants a writable contiguous {want.name} output")
+        if dst.size != batch * dper:
+            raise FftError(-6, f"Mdct: output holds {dst.size} elements, expected {batch} * {dper}")
+        self._lib.check(getattr(self._lib.c, f"b200fft_mdct_{kind}_host")(self._h, src.ctypes.data, dst.ctypes.data, batch))
+        return dst
+
+    def _device(self, kind: str, src, dst, sper: int, dper: int):
+        import torch
+
+        want = torch.float32 if self._precision == F32 else torch.float64
+        if not isinstance(src, torch.Tensor) or src.dtype != want or not src.is_cuda or not src.is_contiguous():
+            raise TypeError(f"Mdct.{kind}_device wants a contiguous CUDA tensor of {want}")
+        if src.numel() % sper:
+            raise FftError(-6, f"Mdct: input holds {src.numel()} elements, expected batch * {sper}")
+        batch = src.numel() // sper
+        if dst is None:
+            shape = (batch, self._frames, self._len) if kind == "forward" else (batch, self._signal_len)
+            dst = torch.empty(shape, dtype=want, device=src.device)
+        if not isinstance(dst, torch.Tensor) or dst.dtype != want or not dst.is_cuda or not dst.is_contiguous():
+            raise TypeError(f"Mdct.{kind}_device wants a contiguous CUDA output tensor of {want}")
+        if src.device.index != self.device or dst.device.index != self.device:
+            raise FftError(-1, f"tensors are on cuda:{src.device.index} / cuda:{dst.device.index}, plan is on cuda:{self.device}")
+        if dst.numel() != batch * dper:
+            raise FftError(-6, f"Mdct: output holds {dst.numel()} elements, expected {batch} * {dper}")
+        coef = dst if kind == "forward" else src
+        if self._pairs and coef.data_ptr() % (2 * coef.element_size()):
+            raise TypeError(f"Mdct.{kind}_device: this plan moves coefficient pairs, so the coefficient tensor must start at an even element")
+        self._lib.check(getattr(self._lib.c, f"b200fft_mdct_{kind}_device")(self._h, src.data_ptr(), dst.data_ptr(), batch,
+                                                                            torch.cuda.current_stream(src.device).cuda_stream))
+        return dst
+
+    def forward(self, x: np.ndarray, out: Optional[np.ndarray] = None) -> np.ndarray:
+        """Every row of `x` (batch * signal_len reals) into `out` (batch * frames * len reals; [batch][frames][len] when None)."""
+        return self._host("forward", x, out, self._signal_len, self._frames * self._len)
+
+    def inverse(self, coefs: np.ndarray, out: Optional[np.ndarray] = None) -> np.ndarray:
+        """Every row of `coefs` (batch * frames * len reals) into `out` (batch * signal_len reals; [batch][signal_len] when None)."""
+        return self._host("inverse", coefs, out, self._frames * self._len, self._signal_len)
+
+    def forward_device(self, x, out=None):
+        """forward on torch CUDA tensors (any shapes, contiguous)."""
+        return self._device("forward", x, out, self._signal_len, self._frames * self._len)
+
+    def inverse_device(self, coefs, out=None):
+        """inverse on torch CUDA tensors (any shapes, contiguous)."""
+        return self._device("inverse", coefs, out, self._frames * self._len, self._signal_len)
+
+
 class DctNd:
     """One planned 2-D or 3-D DCT or DST: the same kind along each of the last len(shape()) axes of contiguous arrays of shape(),
     unnormalised, as scipy.fft.dctn / dstn(x, type, axes=the last r axes) / 2^r, so that Dct3n(Dct2n(x)) = Dst3n(Dst2n(x)) =
@@ -1621,6 +1758,7 @@ class DctPlanner:
         self.device = device
         self._cache: Dict[Tuple[int, int], Dct] = {}
         self._cache_nd: Dict[Tuple[int, Tuple[int, ...]], DctNd] = {}
+        self._cache_mdct: Dict[Tuple[int, bytes, int], Mdct] = {}
         self._lock = threading.Lock()
 
     def plan(self, kind: DctKind, len: int) -> Dct:
@@ -1657,6 +1795,25 @@ class DctPlanner:
 
     def plan_dst4(self, len: int) -> Dct:
         return self.plan(DctKind.Dst4, len)
+
+    def plan_mdct(self, len: int, window, signal_len: int) -> Mdct:
+        """The MDCT of `len` (even) coefficients per frame over rows of signal_len samples; `window` is an array of 2 * len taps or
+        "sine" / "vorbis" (rustdct's window_fn).  Cached per (len, window values, signal_len); see Mdct."""
+        dt = np.float32 if self._precision == F32 else np.float64
+        if isinstance(window, str):
+            w = mdct_window(window, max(int(len), 0), dt)
+        else:
+            if np.iscomplexobj(window):
+                raise TypeError("an MDCT plan needs a real window")
+            w = np.ascontiguousarray(np.asarray(window), dtype=dt)
+            if w.ndim != 1 or w.size != 2 * int(len):
+                raise FftError(-1, f"an MDCT of len {int(len)} needs a 1-D window of {2 * int(len)} taps (got shape {w.shape})")
+        key = (int(len), w.tobytes(), int(signal_len))
+        with self._lock:
+            m = self._cache_mdct.get(key)
+            if m is None:
+                m = self._cache_mdct[key] = Mdct(self._lib, key[0], w, key[2], self._precision, self.device)
+            return m
 
 
 def shard_range(batch: int, rank: int, world: int) -> Tuple[int, int]:

@@ -3,8 +3,9 @@
 # variant (tests/sanitize_conv_check.py), of every 2-D real transform variant (tests/sanitize_real2d_check.py), of every 2-D
 # convolution kernel (tests/sanitize_conv2d_check.py), of every DCT / DST kernel (tests/sanitize_dct_check.py), of every STFT kernel
 # (tests/sanitize_stft_check.py), of the chirp-z transform kernels (tests/sanitize_czt_check.py), of the 3-D plans' axis pass
-# (tests/sanitize_fft3d_check.py), of every multi-channel convolution variant (tests/sanitize_chconv_check.py) and of the
-# analytic-signal kernels (tests/sanitize_hilbert_check.py); logs summarised in $OUT/summary.txt.
+# (tests/sanitize_fft3d_check.py), of every multi-channel convolution variant (tests/sanitize_chconv_check.py), of the
+# analytic-signal kernels (tests/sanitize_hilbert_check.py) and of the MDCT kernels (tests/sanitize_mdct_check.py); logs summarised
+# in $OUT/summary.txt.
 #   default build/switches: memcheck, racecheck, synccheck;  chunked two-pass (B200FFT_FUSED=0): racecheck;
 #   dataflow kernel (B200FFT_FLOW=1): memcheck;  TMA-pipelined one-pass kernels (B200FFT_PIPELINE=1): racecheck
 OUT=${1:-${TMPDIR:-/tmp}/b200fft_sanitize}
@@ -47,6 +48,9 @@ runs tests/sanitize_chconv_check.py chconv_synccheck synccheck
 runs tests/sanitize_hilbert_check.py hilbert_memcheck memcheck
 runs tests/sanitize_hilbert_check.py hilbert_racecheck racecheck
 runs tests/sanitize_hilbert_check.py hilbert_synccheck synccheck
+runs tests/sanitize_mdct_check.py mdct_memcheck memcheck
+runs tests/sanitize_mdct_check.py mdct_racecheck racecheck
+runs tests/sanitize_mdct_check.py mdct_synccheck synccheck
 if [ -z "$SANITIZE_DEFAULT_ONLY" ]; then
 run chunked_racecheck racecheck B200FFT_FUSED=0 SANITIZE_QUICK=1
 run flow_memcheck memcheck B200FFT_FLOW=1 SANITIZE_QUICK=1
