@@ -1,9 +1,10 @@
-"""Every plan family against exact references (tests/exact_cases.py): identity batches against the DFT matrix, impulses and tones
+"""Every plan family against exact references (tests/exact_cases.py, and tests/exact_families.py for the DCT / DST, N-D DCT, STFT,
+chirp-z, 3-D FFT, multi-channel convolution, Hilbert and MDCT plans): identity batches against the DFT matrix, impulses and tones
 against the long-double root table, zero-mean noise against scipy.fft and direct convolution in long double.  One case list, run on
 the CPU replay (unmarked, small sizes) and on the GPU (-m gpu, full sizes).  Seeded and deterministic.
 
 B200FFT_EXACT_REPORT=<path>: after the module, write the worst ratio of each metric and precision (and the case it came from) there
-as JSON -- the figures the docstring of exact_cases.py records."""
+as JSON -- the figures the docstrings of exact_cases.py and exact_families.py record."""
 import json
 import os
 import subprocess
@@ -13,11 +14,14 @@ import numpy as np
 import pytest
 
 import exact_cases as ec
+import exact_families as ef
 from util import ROOT, emu_library
 
 PRECS = pytest.mark.parametrize("prec", (32, 64), ids=("f32", "f64"))
 GROUPS = {"identity": ec.run_identity, "multipass": ec.run_multipass, "real": ec.run_real, "fft2d": ec.run_fft2d,
-          "conv1d": ec.run_conv1d, "conv2d": ec.run_conv2d}
+          "conv1d": ec.run_conv1d, "conv2d": ec.run_conv2d,
+          "dct": ef.run_dct, "dctn": ef.run_dctn, "stft": ef.run_stft, "czt": ef.run_czt, "fft3d": ef.run_fft3d,
+          "chconv": ef.run_chconv, "hilbert": ef.run_hilbert, "mdct": ef.run_mdct}
 
 
 @pytest.fixture(scope="module", autouse=True)
