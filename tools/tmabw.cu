@@ -53,8 +53,9 @@ struct Params {
     CUtensorMap map_in, map_out;  // [slab][rows][cols] with box [1][box_rows][box_cols]
     const char* in;
     char* out;
-    uint32_t tiles;          // tiles in the buffer (tile t: slab t / tiles_per_slab, column block t % tiles_per_slab)
+    uint32_t tiles;          // tiles in the buffer (tile t: part t % split, then column block, then slab)
     uint32_t tiles_per_slab;
+    uint32_t split;          // a column block of the slab is moved as `split` tiles of consecutive rows (adjacent CTAs)
     uint32_t total;          // tiles to move (wraps over `tiles`)
     uint32_t box_cols_elems; // inner box extent in ELEMENTS of the map's data type
     uint32_t box_rows, nbox; // tile = nbox boxes stacked along rows
@@ -87,14 +88,14 @@ __global__ void __launch_bounds__(128, 1) k_tma(const __grid_constant__ Params p
         for (uint32_t t = blockIdx.x; t < p.total; t += gridDim.x, ++i) {
             const uint32_t s = i % NS, ph = (i / NS) & 1u;
             mbar_wait(&empty[s], ph ^ 1u);
-            const uint32_t tt = t % p.tiles;
+            const uint32_t tt = t % p.tiles, cb = tt / p.split, row0 = (tt % p.split) * p.nbox * p.box_rows;
             mbar_expect(&full[s], TILE);
             if (bulk_load)
                 b_g2s(base + s * TILE, p.in + (size_t)tt * TILE, TILE, &full[s]);
             else
                 for (uint32_t k = 0; k < p.nbox; ++k)
-                    t_g2s(base + s * TILE + k * box_bytes, &p.map_in, (int)((tt % p.tiles_per_slab) * p.box_cols_elems), (int)(k * p.box_rows),
-                          (int)(tt / p.tiles_per_slab), &full[s]);
+                    t_g2s(base + s * TILE + k * box_bytes, &p.map_in, (int)((cb % p.tiles_per_slab) * p.box_cols_elems), (int)(row0 + k * p.box_rows),
+                          (int)(cb / p.tiles_per_slab), &full[s]);
         }
     }
     if (threadIdx.x == 32) {  // storer (or the consumer that just frees the stage)
@@ -103,12 +104,12 @@ __global__ void __launch_bounds__(128, 1) k_tma(const __grid_constant__ Params p
             const uint32_t s = i % NS, ph = (i / NS) & 1u;
             if (do_load) mbar_wait(&full[s], ph);
             if (do_store) {
-                const uint32_t tt = t % p.tiles;
+                const uint32_t tt = t % p.tiles, cb = tt / p.split, row0 = (tt % p.split) * p.nbox * p.box_rows;
                 if (bulk_store)
                     b_s2g(p.out + (size_t)tt * TILE, base + s * TILE, TILE);
                 else
                     for (uint32_t k = 0; k < p.nbox; ++k)
-                        t_s2g(&p.map_out, (int)((tt % p.tiles_per_slab) * p.box_cols_elems), (int)(k * p.box_rows), (int)(tt / p.tiles_per_slab),
+                        t_s2g(&p.map_out, (int)((cb % p.tiles_per_slab) * p.box_cols_elems), (int)(row0 + k * p.box_rows), (int)(cb / p.tiles_per_slab),
                               base + s * TILE + k * box_bytes);
                 commit();
                 wait_read0();
@@ -142,9 +143,10 @@ int main() {
     CK(cudaEventCreate(&e0));
     CK(cudaEventCreate(&e1));
     const char* mode_name[8] = {"tensor load", "tensor store", "tensor ld->st", "bulk load", "bulk store", "bulk ld->st", "tensor ld->bulk st", "bulk ld->tensor st"};
-    // tile shapes: rows x row bytes (= 64 KiB), the matrix a slab is cut from has `rows` rows of 8 KiB
-    struct Shape { uint32_t rows, row_bytes; };
-    const Shape shapes[] = {{1024, 64}, {512, 128}, {256, 256}, {128, 512}};
+    // column blocks of a slab (`rows` rows of 8 KiB): rows x row bytes, moved as `split` 64 KiB tiles of rows / split rows each
+    // (1024 x 128 B in two halves: the 16-column block of a 1024-row slab that two adjacent CTAs share)
+    struct Shape { uint32_t rows, row_bytes, split; };
+    const Shape shapes[] = {{1024, 64, 1}, {512, 128, 1}, {1024, 128, 2}, {256, 256, 1}, {128, 512, 1}};
     for (size_t buf : {SMALL, BIG}) {
         for (int esz : {4, 8}) {
             for (const Shape& sh : shapes) {
@@ -153,11 +155,13 @@ int main() {
                 const uint64_t slab_bytes = (uint64_t)sh.rows * slab_row_bytes;
                 const uint64_t slabs = buf / slab_bytes;
                 p.tiles_per_slab = (uint32_t)(slab_row_bytes / sh.row_bytes);
-                p.tiles = (uint32_t)(slabs * p.tiles_per_slab);
+                p.split = sh.split;
+                p.tiles = (uint32_t)(slabs * p.tiles_per_slab * sh.split);
                 p.total = (uint32_t)((4ull << 30) / TILE);
                 p.box_cols_elems = sh.row_bytes / esz;
-                p.box_rows = sh.rows < 256 ? sh.rows : 256;
-                p.nbox = sh.rows / p.box_rows;
+                const uint32_t tile_rows = sh.rows / sh.split;
+                p.box_rows = tile_rows < 256 ? tile_rows : 256;
+                p.nbox = tile_rows / p.box_rows;
                 p.in = a;
                 p.out = b;
                 const cuuint64_t dims[3] = {slab_row_bytes / esz, sh.rows, slabs};
@@ -173,7 +177,7 @@ int main() {
                     return 1;
                 }
                 for (uint32_t mode = 0; mode < 8; ++mode) {
-                    if ((mode == 3 || mode == 4 || mode == 5) && !(esz == 4 && sh.rows == 1024)) continue;  // bulk modes do not depend on the shape
+                    if ((mode == 3 || mode == 4 || mode == 5) && !(esz == 4 && &sh == &shapes[0])) continue;  // bulk modes do not depend on the shape
                     p.mode = mode;
                     float best = 1e30f;
                     for (int r = 0; r < 3; ++r) {
@@ -187,8 +191,8 @@ int main() {
                     }
                     CK(cudaGetLastError());
                     const double bytes = (double)p.total * TILE * ((mode == 2 || mode >= 5) ? 2 : 1);
-                    std::printf("%s  elem %dB  tile %4u x %3uB  %-18s %8.1f GB/s total = %6.1f GB/s per SM (%5.1f B/clk @%.2fGHz)\n", buf == SMALL ? "L2 " : "HBM", esz,
-                                sh.rows, sh.row_bytes, mode_name[mode], bytes / best / 1e6, bytes / best / 1e6 / sms, bytes / best / 1e6 / sms / ghz, ghz);
+                    std::printf("%s  elem %dB  tile %4u x %3uB /%u  %-18s %8.1f GB/s total = %6.1f GB/s per SM (%5.1f B/clk @%.2fGHz)\n", buf == SMALL ? "L2 " : "HBM", esz,
+                                sh.rows, sh.row_bytes, sh.split, mode_name[mode], bytes / best / 1e6, bytes / best / 1e6 / sms, bytes / best / 1e6 / sms / ghz, ghz);
                 }
             }
         }
